@@ -52,22 +52,6 @@ import torch  # noqa: E402
 METRIC = "effective decoded tokens/sec (post-verify) Whisper-large-v2+Medusa"
 REGIMES = {"realistic": 100.0, "mixed0": 260.0, "best": 0.3, "zero": 1.0e6}
 PENALTY = (140, 1.01)          # eval_whisper_medusa.py:61-65 defaults (--regulation-start / --regulation-factor)
-NCU_CAPTURE = os.path.join(ROOT, "profiles", "r2_ring_kernel_ncu.json")
-
-
-def ncu_traffic_bytes(args):
-    """dram__bytes_read.sum + dram__bytes_write.sum of one launch of the dominant kernel, from the committed
-    `ncu --set full` capture of this workload (large-v2, 10 linear heads, persistent mode); null otherwise."""
-    if not (args.preset == "large-v2" and args.heads == 10 and args.heads_type == "base_head" and args.mode == "persistent"):
-        return None
-    for path in (NCU_CAPTURE, os.path.join(ROOT, "profiles", "r1b_ring_kernel_ncu.json")):
-        try:
-            with open(path) as f:
-                pl = json.load(f)["per_launch"]
-            return int(pl["dram_bytes_read"]) + int(pl["dram_bytes_write"])
-        except Exception:  # noqa: BLE001
-            continue
-    return None
 
 
 def algorithmic_bytes(cfg, iterations: int, sweeps_a: int, n_mean: float):
@@ -94,7 +78,7 @@ def algorithmic_bytes(cfg, iterations: int, sweeps_a: int, n_mean: float):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons sampled DURING the timed region."""
 
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
@@ -139,7 +123,7 @@ def measured_peak_gbs():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:  # noqa: BLE001
             pass
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "data sheet (H100 SXM HBM3 3.35 TB/s, not measured)"
 
 
 def cpu_threads() -> int:
@@ -203,6 +187,19 @@ def run_streams(model, clips, idx, language, alpha, max_iters=0):
     return traces, outs, time.perf_counter() - t0
 
 
+def dump_outputs(path, model, tokens, trace):
+    """The last timed step's results, as a caller of generate_from_pcm receives them: the token ids, the full sequence
+    and accept lengths of the trace, plus the state they were computed from -- the encoder output and the raw logits of
+    the last verify pass (both fp32, a few MB at large-v2).  Token ids are exact in float64."""
+    os.makedirs(path, exist_ok=True)
+    arrays = {"tokens": np.asarray(tokens, np.float64), "sequences": np.asarray(trace.sequences, np.float64),
+              "accept_lengths": np.asarray(trace.accept_lengths, np.float64),
+              "encoder_output": model.encoder_output().numpy().astype(np.float32),
+              "last_logits_verify": model.last_logits(1).numpy().astype(np.float32)}
+    for name, a in arrays.items():
+        np.save(os.path.join(path, name + ".npy"), a)
+
+
 def summarize(cfg, traces, peak):
     toks = sum(t.n_new_tokens for t in traces)
     iters = sum(t.iterations for t in traces)
@@ -238,6 +235,9 @@ def main():
     ap.add_argument("--streams", type=int, default=4,
                     help="concurrent streams per GPU of the multi-stream measurement (detail.multi_stream; BASELINE configs[3])")
     ap.add_argument("--dump-tokens", default=None, help="write this rank's token lists (JSON) to PATH.rank<r>")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write what the last timed step returned (rank 0) as DIR/<name>.npy, for output-by-output "
+                         "comparison of two builds")
     args = ap.parse_args()
 
     from whisper_medusa_b200.synthetic import preset_config, synthetic_audio, synthetic_state_dict
@@ -254,7 +254,7 @@ def main():
     config = {"workload": workload, "acceptance_regime": f"{args.regime} (posterior_alpha={alpha:g})",
               "streams_per_step": world, "parallelism": f"replicas x{world} (independent streams)",
               "weights": "seeded synthetic fp16 (seed 0)",
-              "l2": "weights (3.1 GB) >> L2 (126 MB): every iteration re-streams them from HBM"}
+              "l2": "weights (3.1 GB) >> L2 (50 MB): every iteration re-streams them from HBM"}
     threads = cpu_threads()
 
     # ------------------------------------------------------------------ reference arm (CPU oracle)
@@ -339,6 +339,8 @@ def main():
     if args.dump_tokens:
         with open(f"{args.dump_tokens}.rank{rank}", "w") as f:
             json.dump({"stream_ids": [rank + world * i for i in range(args.steps)], "tokens": outs}, f)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, model, outs[-1], traces[-1])
 
     stats = torch.tensor([sm["tokens"], sm["iterations"], sm["ms_decode"], wall, enc_ms, mel_ms, launches], dtype=torch.float64, device=device)
     if dist is not None:
@@ -433,7 +435,7 @@ def main():
         "gpu_launches": int(allv[:, 6].sum()),
         "clocks": clocks,
         "roofline": {"bound": "hbm", "achieved": sm["achieved_gbs"], "peak": peak, "unit": "GB/s", "frac": sm["frac"],
-                     "traffic": ncu_traffic_bytes(args), "peak_source": peak_src,
+                     "peak_source": peak_src,
                      "kernel": "dec_iteration_ring_kernel (one launch = one speculative iteration)"
                      if args.mode == "persistent" else f"decode iteration ({args.mode})",
                      "algorithmic_bytes_per_iteration": sm["bytes_eng"] / max(1, sm["iterations"]),

@@ -1,5 +1,5 @@
 /*
- * whisper_medusa_b200 -- C ABI of the B200-native Whisper-Medusa decode path.
+ * whisper_medusa_b200 -- C ABI of the H100-native Whisper-Medusa decode path.
  *
  * The reference (aiola-lab/whisper-medusa) is pure Python and has no FFI of its own; the
  * boundary it exposes for this path is the Python surface of
@@ -141,15 +141,15 @@ int wm_set_decode_mode(wm_handle* h, int32_t mode);
  * instead of holding its own copy -- how S concurrent streams share one blob. */
 void* wm_weights_device_ptr(wm_handle* h);
 /* Engine options: "decode_ctas" = CTAs of the decode grid (default: every SM; S handles with n_sm / S each decode S
- * streams concurrently -- SURVEY 8(f) rank 3, the reference is batch 1 at model.py:1451); "decode_mode" (as above); "enc_gemm" 1 = tcgen05/TMA/TMEM encoder GEMM (default),
- * 0 = mma.sync encoder GEMM (cross-check), 2 = tcgen05 with 128-row tiles only (cross-check of the per-GEMM tile
- * shapes); "enc_attn" 1 = tcgen05/TMA/TMEM encoder attention (default), 0 = mma.sync flash attention (cross-check);
+ * streams concurrently -- SURVEY 8(f) rank 3, the reference is batch 1 at model.py:1451); "decode_mode" (as above); "enc_gemm" 1 = wgmma/TMA encoder GEMM (default),
+ * 0 = mma.sync encoder GEMM (cross-check), 2 = wgmma with 128 x 128 tiles only (cross-check of the per-GEMM tile
+ * shapes); "enc_attn" 1 = wgmma/TMA encoder attention (default), 0 = mma.sync flash attention (cross-check);
  * "enc_pdl" 1 = encoder kernels under programmatic dependent launch (default), 0 = plain stream-ordered launches;
  * "profile" 1 = record the stage timeline below. */
 int wm_set_option(wm_handle* h, const char* key, int32_t value);
-/* Host logic, no GPU needed: the tile {rows, columns, ring stages} the tcgen05 encoder GEMM runs an M x N x K product
- * with on a GPU of n_sm SMs (0: 148) -- the shape with the fewest operand bytes on the busiest SM (DESIGN.md section 4).
- * fp16_out: the bias / bias+GELU epilogues; 0: the fp32 residual-stream epilogues (128-row tiles only). */
+/* Host logic, no GPU needed: the tile {rows, columns, ring stages} the wgmma encoder GEMM runs an M x N x K product
+ * with on a GPU of n_sm SMs (0: 132) -- the shape with the fewest operand bytes on the busiest SM (DESIGN.md section 4).
+ * fp16_out: the bias / bias+GELU epilogues; 0: the fp32 residual-stream epilogues (128 x 128 tiles only). */
 int wm_enc_gemm_tile(int32_t M, int32_t N, int32_t K, int32_t fp16_out, int32_t n_sm, int32_t* out3);
 /* Debug: per-stage timeline of the last persistent iteration (after wm_set_option(h, "profile", 1)).
  * Rows of 24 int64: stage id, mode, layer; body ns and barrier-wait ns seen by the last CTA; then the

@@ -8,7 +8,7 @@ Streams are NOT selected: seed s of every group is simply ``base_seed + s``.  Fo
 the reference's full ``input_ids`` (prompt + emitted tokens + post-EOS fill) and its accept-length list,
 fp32 on CPU.  Consumers:
   * tests/test_ref_loop_pin.py (CPU): the oracle restatement reproduces every stream bit-for-bit;
-  * tests/test_gpu_parity.py  (B200): the CUDA engine against the same streams -- mismatch RATE over all
+  * tests/test_gpu_parity.py  (H100): the CUDA engine against the same streams -- mismatch RATE over all
     of them (fp16-operand rounding can flip a near-tie; a flipped decision changes the rest of the stream).
 """
 from __future__ import annotations

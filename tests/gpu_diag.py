@@ -2,7 +2,7 @@
 
     python tests/gpu_diag.py [case ...] [--mode graph|persistent] [--large]
 
-Prints one line per check (never raises on a numeric mismatch) so a single gpurun call shows
+Prints one line per check (never raises on a numeric mismatch) so a single GPU run shows
 where a divergence starts: mel -> encoder -> first-iteration logits -> token ids.
 """
 from __future__ import annotations
@@ -46,7 +46,7 @@ def run_case(name: str, mode: str, use_oracle: bool = True):
     model = WhisperMedusaModel(cfg, sd).to("cuda:0")
     model.set_decode_mode(mode)
     if TC:
-        model.set_option("enc_gemm", 1)   # tcgen05 / TMA / TMEM encoder GEMM
+        model.set_option("enc_gemm", 1)   # wgmma / TMA encoder GEMM
     print(f"[{name}/{mode}] setup {time.time() - t0:.1f}s", flush=True)
     language = "en" if cfg.is_multilingual else None
     kw = dict(language=language, max_length=max_len, exponential_decay_length_penalty=pen, medusa_temperature=temp)

@@ -3,7 +3,7 @@
     python tests/gpu_stage_profile.py [--preset large-v2] [--heads 10] [--block] [--iters 6] [--tc] [--temp0] [--seed 0]
 
 Prints, per stage type, the mean body time and barrier-wait time over the layers of the LAST
-iteration, and the critical-path sum.  Used to decide what to optimise next (profiles/*.txt).
+iteration, and the critical-path sum.  Used to decide what to optimise next.
 """
 from __future__ import annotations
 

@@ -1,6 +1,6 @@
 """Concurrent streams on one GPU (development aid / measurement; the test is in test_gpu_parity.py).
 
-    python tests/gpu_streams.py [--preset large-v2] [--heads 10] [--clips 8] [--configs 1x148,2x74,4x37] [--alpha 100]
+    python tests/gpu_streams.py [--preset large-v2] [--heads 10] [--clips 8] [--configs 1x132,2x66,4x33] [--alpha 100]
 
 For every configuration SxC (S engines sharing one weight blob, C CTAs each): runs the clips, checks every clip's tokens
 against the single-stream run, prints ms per iteration per stream, aggregate tokens/s and achieved HBM GB/s
@@ -30,7 +30,7 @@ def arg(name, default):
 def main():
     preset, heads, n_clips = arg("--preset", "large-v2"), arg("--heads", 10), arg("--clips", 8)
     alpha = arg("--alpha", 100.0)
-    configs = [tuple(int(v) for v in c.split("x")) for c in arg("--configs", "1x148,2x74,4x37").split(",")]
+    configs = [tuple(int(v) for v in c.split("x")) for c in arg("--configs", "1x132,2x66,4x33").split(",")]
     cfg = preset_config(preset, heads=heads)
     sd = synthetic_state_dict(cfg, seed=0)
     secs = 30.0 if preset == "large-v2" else 5.0

@@ -1,7 +1,7 @@
-"""Per-kernel SASS mnemonic counts of the in-tree engine library (evidence that the tcgen05 / TMA / TMEM paths are the
-ones compiled in; B200_PROFILING.md lists the mnemonics).  No GPU needed:
+"""Per-kernel SASS mnemonic counts of the in-tree engine library (evidence that the wgmma / TMA paths are the ones
+compiled in).  No GPU needed:
 
-    python tests/sass_summary.py > profiles/r2_sass_summary.txt
+    python tests/sass_summary.py
 """
 from __future__ import annotations
 
@@ -13,7 +13,7 @@ import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 LIB = os.path.join(ROOT, "whisper_medusa_b200", "_lib", "libwm_b200.so")
-WATCH = ["UTCHMMA", "UTCQMMA", "UTCBAR", "UTCATOMSWS", "UTMALDG", "UTMASTG", "UTMAPF", "LDTM", "STTM", "UBLKCP", "SYNCS", "HMMA",
+WATCH = ["HGMMA", "WARPGROUP", "UTMALDG", "UTMASTG", "UTMAPF", "UBLKCP", "SYNCS", "HMMA",
          "LDGSTS", "LDSM", "REDG", "ATOMG", "MEMBAR", "ERRBAR", "CCTL", "BAR", "UCGABAR", "MUFU", "LDG", "STG", "LDS", "STS"]
 
 
@@ -44,8 +44,8 @@ def main():
                 if op == w or op.startswith(w):
                     kernels[cur][w] += 1
                     break
-    print(f"# cuobjdump -sass {os.path.relpath(LIB, ROOT)}: instruction counts per kernel (static), sm_100a")
-    print("# tcgen05 = UTCHMMA (MMA) / UTCBAR (commit) / LDTM, STTM (TMEM load/store); TMA tensor copies = UTMALDG / UTMASTG;")
+    print(f"# cuobjdump -sass {os.path.relpath(LIB, ROOT)}: instruction counts per kernel (static), sm_90a")
+    print("# wgmma = HGMMA (MMA) / WARPGROUP (arrive, depbar); TMA tensor copies = UTMALDG / UTMASTG;")
     print("# bulk (non-tensor) async copies = UBLKCP; mbarrier = SYNCS; legacy tensor-core MMA = HMMA; cp.async = LDGSTS")
     for k, c in kernels.items():
         name = demangle(k)

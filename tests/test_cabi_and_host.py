@@ -34,31 +34,31 @@ def test_strerror_and_null_handles(engine_lib):
 
 def test_encoder_gemm_tile_choice(engine_lib):
     """Host logic of csrc/enc_gemm_tc.cu::pick_tile: the tile with the fewest operand bytes, K (BM + BN) 2 per tile x
-    ceil(tiles / n_sm) tiles, on the busiest SM (these GEMMs are bound by the per-SM L2 -> shared-memory rate, DESIGN.md
-    section 4).  whisper-large-v2 (M = 1500 positions, 148 SMs): every GEMM runs as ONE wave of 120 tiles."""
-    def tile(M, N, K, fp16_out, n_sm=148):
+    ceil(tiles / n_sm) tiles, on the busiest SM.  whisper-large-v2 (M = 1500 positions) on the 132 SMs of an H100: the
+    wide GEMMs run in at most two rounds of tiles."""
+    def tile(M, N, K, fp16_out, n_sm=132):
         out = (C.c_int32 * 3)()
         assert engine_lib.wm_enc_gemm_tile(M, N, K, int(fp16_out), n_sm, out) == 0
         return tuple(out)
 
-    assert tile(1500, 3840, 1280, True) == (256, 192, 4)     # QKV: 6 x 20 tiles
-    assert tile(1500, 5120, 1280, True) == (256, 256, 3)     # FC1: 6 x 20
+    assert tile(1500, 3840, 1280, True) == (128, 192, 5)     # QKV: 12 x 20 tiles
+    assert tile(1500, 5120, 1280, True) == (256, 128, 4)     # FC1: 6 x 40
     assert tile(1500, 2560, 1280, True) == (256, 128, 4)     # cross-K/V: 6 x 20
     assert tile(1500, 1280, 1280, False) == (128, 128, 6)    # O-proj: 12 x 10, one CTA per SM, deep ring
     assert tile(1500, 1280, 5120, False) == (128, 128, 6)    # FC2
     assert tile(3000, 1280, 256, True) == (256, 128, 4)      # conv1 as an implicit GEMM: 12 x 10
-    # tiny (d = 384): every output is narrow, 128-row tiles already fit one wave
+    # tiny (d = 384): 128 x 128 tiles fit one round where N <= 1408; FC1 (N = 1536) takes 128 x 192 instead
     assert tile(1500, 1152, 384, True)[:2] == (128, 128)
-    assert tile(1500, 1536, 384, True)[:2] == (128, 128)
+    assert tile(1500, 1536, 384, True)[:2] == (128, 192)
     # the cost model itself: no candidate may beat the chosen tile
     for (M, N, K) in [(1500, 3840, 1280), (1500, 5120, 1280), (1500, 2560, 1280), (1500, 2048, 512), (700, 3072, 768)]:
         bm, bn, _ = tile(M, N, K, True)
-        cost = lambda a, b: -(-((-(-M // a)) * (N // b)) // 148) * (a + b)
-        for a, b in [(128, 128), (256, 128), (256, 192), (256, 256)]:
+        cost = lambda a, b: -(-((-(-M // a)) * (N // b)) // 132) * (a + b)
+        for a, b in [(128, 128), (256, 128), (128, 192), (128, 256)]:
             if N % b == 0:
                 assert cost(bm, bn) <= cost(a, b), (M, N, K, bm, bn, a, b)
-    assert engine_lib.wm_enc_gemm_tile(1500, 1000, 1280, 1, 148, (C.c_int32 * 3)()) != 0   # N must be a multiple of 128
-    assert engine_lib.wm_enc_gemm_tile(1500, 1280, 1280, 1, 148, None) != 0
+    assert engine_lib.wm_enc_gemm_tile(1500, 1000, 1280, 1, 132, (C.c_int32 * 3)()) != 0   # N must be a multiple of 128
+    assert engine_lib.wm_enc_gemm_tile(1500, 1280, 1280, 1, 132, None) != 0
 
 
 def _layout_handle(lib, cfg):

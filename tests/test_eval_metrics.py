@@ -1,7 +1,6 @@
 """WER / CER restatement (whisper_medusa_b200/metrics.py, reference whisper_medusa/utils/metrics.py:5-71 on
 jiwer 3.0.3) and the evaluation driver (whisper_medusa_b200/eval.py, reference eval_whisper_medusa.py:21-96).
 jiwer is not installed here, so the known answers below are worked by hand from its documented transforms."""
-import os
 import struct
 import wave
 
@@ -100,28 +99,3 @@ def test_audio_loading_and_driver(tmp_path):
     assert table["wer"] == pytest.approx([0.5, 0.0, 0.0])
     assert wer == pytest.approx(1 / 5)          # 1 error over 2 + 2 + 1 ("EMPTY") words
     assert 0 < cer < 0.1
-
-
-def test_scores_match_the_reference_metrics_when_jiwer_is_installed():
-    """Optional pin (ADVICE r1): where jiwer and the reference checkout exist, the restated transform chains must give
-    the scores of the reference's own utils/metrics.py on a corpus with contractions, Kaldi tags, unicode punctuation and
-    empty strings.  (Neither is available in the authoring container: the test is skipped there.)"""
-    import importlib.util
-
-    pytest.importorskip("jiwer")
-    ref_path = "/root/reference/whisper_medusa/utils/metrics.py"
-    if not os.path.isfile(ref_path):
-        pytest.skip("reference checkout not present")
-    spec = importlib.util.spec_from_file_location("ref_metrics", ref_path)
-    ref = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(ref)
-    from whisper_medusa_b200 import metrics as ours
-
-    preds = ["I can't  go, it's late!", "<unk> hello [noise] world", "", "“Quoted” — text…", "the cat sat"]
-    refs = ["i cannot go it is late", "hello world", "something", "quoted text", ""]
-    rw, rws = ref.compute_wer(preds, refs)
-    ow, ows = ours.compute_wer(preds, refs)
-    rc, rcs = ref.compute_cer(preds, refs)
-    oc, ocs = ours.compute_cer(preds, refs)
-    assert abs(rw - ow) < 1e-12 and abs(rc - oc) < 1e-12
-    assert np.allclose(rws, ows) and np.allclose(rcs, ocs)

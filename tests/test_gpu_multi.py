@@ -1,6 +1,6 @@
 """N-rank run == N single-GPU runs (SURVEY.md section 4): the 2-rank NCCL launch of bench.py (weights broadcast from
 rank 0 over NVLink, streams sharded rank + world * i) must return, for every stream, exactly the tokens one GPU
-returns for that stream.  Needs two GPUs: `gpurun --gpus 2 -- python -m pytest tests/test_gpu_multi.py -m gpu`."""
+returns for that stream.  Needs two GPUs: `python -m pytest tests/test_gpu_multi.py -m gpu` on a machine with two or more."""
 import json
 import os
 import subprocess

@@ -126,7 +126,7 @@ def test_mel_encoder_logits_close(name, mode):
 
 @pytest.mark.parametrize("name", ["micro_linear_k4", "tiny_linear_k4"])
 def test_encoder_gemm_implementations_agree(name):
-    """The encoder GEMMs run on the tcgen05 / TMA / TMEM kernel by default; the mma.sync kernel
+    """The encoder GEMMs run on the wgmma / TMA kernel by default; the mma.sync kernel
     (option enc_gemm = 0) is the cross-check: same fp16 operands, fp32 accumulation in a different
     order => the outputs agree to the fp16-rounding-flip level (DESIGN.md section 2) and both stay
     within the oracle tolerance; the tokens are identical."""
@@ -153,7 +153,7 @@ def test_encoder_gemm_implementations_agree(name):
 
 @pytest.mark.parametrize("name", ["micro_linear_k4", "tiny_linear_k4"])
 def test_encoder_attention_implementations_agree(name):
-    """Encoder self-attention runs on the tcgen05 / TMA / TMEM kernel by default (enc_attn_tc.cu); the mma.sync flash
+    """Encoder self-attention runs on the wgmma / TMA kernel by default (enc_attn_tc.cu); the mma.sync flash
     attention (option enc_attn = 0) is the cross-check: same 64-key blocking and fp16 rounding of P, fp32 accumulation
     in a different order => encoder states agree to the fp16-rounding-flip level, both within the oracle tolerance, and
     the tokens are identical."""
@@ -237,9 +237,8 @@ def test_large_v2_tokens_bit_exact_vs_golden(mode):
             lg = model.last_logits(which).numpy()
             assert _rel_err(lg, ref.numpy()) < 1e-3, ab
             assert _rel_err(lg[:, ::97], g[f"logits{ab}0_strided"]) < 5e-3, ab
-        # tcgen05 GEMM tile shapes: at d = 1280 the wide outputs run as 256 x 192 / 256 x 256 / 256 x 128 tiles (two
-        # 128-row accumulators per CTA); option enc_gemm = 2 forces 128-row tiles.  Same operands, same K order per
-        # output element => identical encoder states.
+        # wgmma GEMM tile shapes: at d = 1280 the wide outputs run as 128 x 192 / 256 x 128 tiles; option enc_gemm = 2
+        # forces 128 x 128 tiles.  Same operands, same K order per output element => identical encoder states.
         model.set_option("enc_gemm", 2)
         model.generate_from_pcm(pcm, max_iters=1, **kw)
         enc128 = model.encoder_output()
@@ -304,11 +303,14 @@ def test_large_v2_mixed_acceptance_tokens_bit_exact(name):
 
 def test_engine_vs_the_reference_loop_on_unselected_streams():
     """The CUDA engine against outputs of the REFERENCE'S OWN loop code (tests/golden/ref_loop_streams.npz, made by
-    oracle/make_ref_golden.py from /root/reference): 82 streams whose seeds were not selected for decision margins.
+    oracle/make_ref_golden.py from the reference checkout): 82 streams whose seeds were not selected for decision margins.
     The engine computes with fp16 K/V caches and fp16 hi/lo operands, the reference in fp32, so a decision that sits
     within ~1e-3 of a tie can flip (and changes the rest of that stream).  Asserted: a stream either matches the
     reference bit-for-bit or matches the oracle run in the engine's rounding regime on the same inputs (i.e. the
-    difference is the numeric regime, not the algorithm); and the mismatch RATE against the reference stays small."""
+    difference is the numeric regime, not the algorithm); and the mismatch RATE against the reference stays small.
+    The oracle's encoder sums in another order than the engine's tensor-core tiles, so a decode decision within that
+    rounding noise of a tie can also separate the engine from the oracle's own encoder states: such a stream must then
+    match the oracle decoding from the engine's encoder states (as in the branching-tree and prefill tests)."""
     from oracle import make_ref_golden as G
     from whisper_medusa_b200 import WhisperMedusaModel
 
@@ -322,6 +324,7 @@ def test_engine_vs_the_reference_loop_on_unselected_streams():
             m.generate_from_pcm(pcm, max_length=max_len, exponential_decay_length_penalty=pen, medusa_temperature=temp,
                                 posterior_alpha=alpha, posterior_threshold=thr)
             seq, acc = m.last_trace.sequences, m.last_trace.accept_lengths
+            enc_engine = m.encoder_output()
             m.close()
             total += 1
             if seq == fx[f"{group}/{s}/sequences"].tolist() and acc == fx[f"{group}/{s}/accept"].tolist():
@@ -333,7 +336,10 @@ def test_engine_vs_the_reference_loop_on_unselected_streams():
             prompt = M.init_tokens(cfg, None)
             gp = M.gen_params(cfg, prompt, pen, max_len, temperature=temp, posterior_alpha=alpha, posterior_threshold=thr)
             tr = M.medusa_greedy_search(w, cfg, enc, prompt, gp, "engine")
-            report.append((group, s, seq == tr.sequences))
+            same_encoder = seq == tr.sequences and acc == tr.accept_lengths
+            if not same_encoder:
+                tr = M.medusa_greedy_search(w, cfg, enc_engine, prompt, gp, "engine")
+            report.append((group, s, "oracle" if same_encoder else "oracle from the engine's encoder states"))
             assert seq == tr.sequences and acc == tr.accept_lengths, (group, s)
     print(f"engine vs reference loop: {mism} of {total} streams differ (numeric-regime flips: {report})")
     assert total >= 80 and mism <= total // 10, (mism, total, report)

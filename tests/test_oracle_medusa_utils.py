@@ -1,24 +1,19 @@
-"""Pins the oracle's restatement of medusa_utils.py against the reference file itself (loaded by
-path; only where /root/reference exists, i.e. the authoring container) and against known answers
+"""Pins the oracle's restatement of medusa_utils.py against what the reference file itself returns for the same inputs
+(frozen in tests/golden/reference/medusa_utils.npz by oracle/make_medusa_utils_golden.py) and against known answers
 recorded from it (SURVEY.md section 4)."""
-import importlib.util
 import os
 
+import numpy as np
 import pytest
 import torch
 
+from _wm_paths import GOLDEN
+from oracle import make_medusa_utils_golden as G
 from oracle import medusa_ref as M
-
-REF = "/root/reference/whisper_medusa/models/medusa_utils.py"
 
 
 def _ref():
-    if not os.path.isfile(REF):
-        pytest.skip("reference checkout not present on this box")
-    spec = importlib.util.spec_from_file_location("ref_medusa_utils", REF)
-    m = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(m)
-    return m
+    return np.load(os.path.join(GOLDEN, "reference", "medusa_utils.npz"))
 
 
 def test_buffers_known_answer():
@@ -33,45 +28,34 @@ def test_buffers_known_answer():
     assert c["retrieve_indices"].tolist() == [list(range(11))]
 
 
-@pytest.mark.parametrize("choices", [[1, 1, 1, 1, 1], [1] * 11, [1, 2, 2], [1, 3, 2, 1], [1, 6, 5, 4, 3]])
+@pytest.mark.parametrize("choices", G.BUFFER_CHOICES)
 def test_buffers_match_reference(choices):
-    r = _ref().generate_medusa_buffers(choices, device="cpu")
+    r = _ref()
     o = M.generate_medusa_buffers(choices)
     for k in ("tree_indices", "medusa_position_ids", "retrieve_indices"):
-        assert torch.equal(r[k].long(), o[k].long()), k
+        assert torch.equal(torch.from_numpy(r[f"buffers/{G.key(choices)}/{k}"]), o[k].long()), k
 
 
-@pytest.mark.parametrize("choices", [[1, 1, 1, 1, 1], [1, 2, 2], [1, 3, 2, 1]])
+@pytest.mark.parametrize("choices", G.CANDIDATE_CHOICES)
 def test_candidates_match_reference(choices):
-    ref = _ref()
-    g = torch.Generator().manual_seed(7)
-    H, V, T = len(choices) - 1, 300, 3
-    med = torch.randn(H, 1, T, V, generator=g)
-    base = torch.randn(1, T, V, generator=g)
+    r = _ref()
+    med, base = G.candidate_inputs(choices)
     bufs = M.generate_medusa_buffers(choices)
-    rc, rt = ref.generate_candidates(med, base, choices[1:], bufs["tree_indices"])
     oc, ot = M.generate_candidates(med[:, 0, -1], base[0, -1], choices[1:], bufs["tree_indices"])
-    assert torch.equal(rc, oc)
-    assert torch.equal(rt[0], ot)
+    assert torch.equal(torch.from_numpy(r[f"candidates/{G.key(choices)}/cart"]), oc.long())
+    assert torch.equal(torch.from_numpy(r[f"candidates/{G.key(choices)}/tree"]), ot.long())
 
 
-@pytest.mark.parametrize("temperature", [0.0, 1.0, 0.7])
-@pytest.mark.parametrize("choices", [[1, 1, 1, 1, 1], [1, 2, 2]])
+@pytest.mark.parametrize("temperature", G.POSTERIOR_TEMPERATURES)
+@pytest.mark.parametrize("choices", G.POSTERIOR_CHOICES)
 def test_evaluate_posterior_matches_reference(choices, temperature):
-    ref = _ref()
-    g = torch.Generator().manual_seed(3)
-    bufs = M.generate_medusa_buffers(choices)
-    n_cand, depth = bufs["retrieve_indices"].shape
-    V = 200
-    for trial in range(40):
-        logits = torch.randn(n_cand, depth, V, generator=g) * (0.5 + trial % 4)
-        cands = torch.randint(0, V, (n_cand, depth), generator=g)
-        if trial % 3 == 0:  # make some prefixes match the argmax so accepts happen
-            cands[:, 1:] = logits[:, :-1].argmax(-1)
-            cands[:, 1 + trial % depth:] = 0
-        rb, ra = ref.evaluate_posterior(logits, cands, temperature, 0.09, 0.3)
+    want = _ref()[f"posterior/{G.key(choices)}/{temperature}"]
+    n_cand, depth = M.generate_medusa_buffers(choices)["retrieve_indices"].shape
+    inputs = G.posterior_inputs(n_cand, depth)
+    assert len(want) == len(inputs) == G.POSTERIOR_TRIALS
+    for (logits, cands), (rb, ra) in zip(inputs, want.tolist()):
         ob, oa = M.evaluate_posterior(logits, cands, temperature, 0.09, 0.3)
-        assert int(ra) == oa and int(rb) == ob
+        assert ra == oa and rb == ob
 
 
 def test_processors_match_hf():

@@ -1,4 +1,4 @@
-"""B200-native Whisper-Medusa decode path behind the reference's Python API.
+"""H100-native Whisper-Medusa decode path behind the reference's Python API.
 
 ``from whisper_medusa_b200 import WhisperMedusaModel`` mirrors
 ``from whisper_medusa import WhisperMedusaModel`` (reference ``whisper_medusa/__init__.py:1``).

@@ -1,4 +1,4 @@
-"""In-tree build of the CUDA engine: nvcc -> whisper_medusa_b200/_lib/libwm_b200.so (sm_100a only).
+"""In-tree build of the CUDA engine: nvcc -> whisper_medusa_b200/_lib/libwm_b200.so (sm_90a only).
 
 ``python -m whisper_medusa_b200.build`` or ``__graft_entry__.build()``.  Objects are rebuilt only
 when a source or header is newer.  nvcc cross-compiles without a GPU.
@@ -22,7 +22,7 @@ ROOT = os.path.dirname(HERE)
 SOURCES = ["engine.cu", "decode.cu", "mel.cu", "enc_gemm.cu", "enc_attn.cu", "enc_gemm_tc.cu", "enc_attn_tc.cu"]
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC", "-Xptxas", "-v",
     # the stage-sequence templates are __host__ __device__ and are instantiated with host lambdas on
     # the host side only; nvcc warns about the (never taken) device instantiation
@@ -78,7 +78,7 @@ def build(verbose: bool = False, force: bool = False, extra_flags: List[str] = (
         if verbose:
             print(log)
     if force or _newer(objs, lib_path):
-        cmd = [nvcc, "-shared", "-o", lib_path] + objs + ["-gencode", "arch=compute_100a,code=sm_100a", "-lcudart"]
+        cmd = [nvcc, "-shared", "-o", lib_path] + objs + ["-gencode", "arch=compute_90a,code=sm_90a", "-lcudart"]
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:
             raise RuntimeError(f"link failed:\n{r.stdout}\n{r.stderr}")

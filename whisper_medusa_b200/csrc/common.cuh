@@ -1,4 +1,4 @@
-// Shared device helpers and engine-internal types (sm_100a only).
+// Shared device helpers and engine-internal types (sm_90a only).
 #pragma once
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>

@@ -1,4 +1,4 @@
-// Decode-side kernels of the Medusa speculative loop (sm_100a).
+// Decode-side kernels of the Medusa speculative loop (sm_90a).
 //
 // One speculative iteration = pass A (the not-yet-cached token(s), all K+1 heads) followed by
 // pass B (verify: the K+1 candidate tokens, base head only) -- reference model.py:635-793 and

@@ -136,7 +136,7 @@ __host__ __device__ __forceinline__ GemmWork gemm_work(int N, int K, int d, int 
 __host__ __device__ constexpr size_t cmax(size_t a, size_t b) { return a > b ? a : b; }
 __host__ __device__ constexpr size_t round128(size_t a) { return (a + 127) / 128 * 128; }
 #ifndef WM_RING_NKS_MAX
-#define WM_RING_NKS_MAX 4   /* A/B round 2 (large-v2, ms per iteration): 8 MMA warps 1.887, 5: 1.900, 4: 1.859, 2: 2.059 */
+#define WM_RING_NKS_MAX 4   /* MMA warps per GEMM stage (k-slices); chosen by A/B timing at large-v2 */
 #endif
 __host__ __device__ constexpr int ring_nks(int d) {
 #ifdef WM_RING_NKS_FORCE
@@ -519,7 +519,7 @@ __device__ __forceinline__ void stage_gemm_ring(RingState& rs, unsigned char* sm
           out[(size_t)token * ldo + row] = xbuf_value(xb, G::XS, token, row) + silu(s + bias_v[k]);
         }
       }
-      if (u + 1 < units) fetch(u + 1, bias_v, old);   // (A/B round 2: fetching TWO units ahead into a second register set was slower, 1.932 vs 1.905 ms)
+      if (u + 1 < units) fetch(u + 1, bias_v, old);   // (fetching TWO units ahead into a second register set timed slower)
     }
     for (int u = 0; u < units; ++u)
       if (++rs.slot == WM_RING_G) { rs.slot = 0; rs.par ^= 1u; }   // keep the (uniform) ring state in step with the MMA warps

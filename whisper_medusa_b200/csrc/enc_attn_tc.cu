@@ -1,19 +1,17 @@
-// Encoder self-attention on the 5th-generation tensor cores (sm_100a): full (non-causal) softmax(Q K^T / 8) V over
+// Encoder self-attention on the Hopper tensor cores (sm_90a, wgmma): full (non-causal) softmax(Q K^T / 8) V over
 // S = 1500 positions, head_dim 64 (HF modeling_whisper.py:284-357).  Same blocking and rounding points as the mma.sync
 // kernel (enc_attn.cu: 64-key blocks, online softmax in fp32 with exp2, un-normalised P rounded to fp16 for the P V
 // product, fp32 O), so the two agree to fp32 accumulation order and enc_attn.cu stays the cross-check.
 //
 // One CTA = one head x 128 query rows, two CTAs per SM.
-//   warp 0      : TMA producer -- Q tile once, then per key block the K tile [64 keys][64] and the V^T tile
+//   warp 8      : TMA producer -- Q tile once, then per key block the K tile [64 keys][64] and the V^T tile
 //                 [64 dims][64 keys] (cp.async.bulk.tensor.2d, SWIZZLE_128B) into a 3-stage ring
-//   warp 1      : MMA issuer   -- S_b = Q K^T (tcgen05.mma M=128 N=64, 4 x K=16) into one of two TMEM score buffers,
-//                 D = P_b V (M=128 N=64, 4 x K=16, P_b from shared memory) into a TMEM block-output buffer;
-//                 tcgen05.commit signals the softmax warps / frees the ring stage
-//   warps 2..9  : softmax      -- two threads per query row (TMEM lane quarter = warp % 4, 32 key columns / 32 output
-//                 dims each): tcgen05.ld of the scores, running max / sum, P as
-//                 fp16 into a double-buffered shared tile in the UMMA K-major SWIZZLE_128B layout, O (32 fp32 registers)
-//                 rescaled and accumulated from D
-// V^T ([H*64][S_pad] fp16) is produced by enc_transpose_v_kernel so that both products use K-major operands.
+//   warps 0-7   : two consumer warpgroups of 64 query rows each: S = Q K^T (wgmma m64n64k16 x4, both operands in shared
+//                 memory) into registers, online softmax on the accumulator fragments (a row is spread over the 4
+//                 threads of a quad), P rounded to fp16 in registers in the A-fragment layout, O += P V^T (wgmma
+//                 m64n64k16 x4, A from registers); the ring stage is released once both products have completed
+// V^T ([H*64][S_pad] fp16) is written by the QKV GEMM's epilogue or by enc_transpose_v_kernel, so that both products
+// use K-major operands.
 #include <cuda.h>
 
 #include <map>
@@ -28,13 +26,10 @@ namespace wm {
 #define AT_BQ 128
 #define AT_BK 64
 #define AT_STAGES 3
-#define AT_THREADS 320
-#define AT_TMEM_COLS 256
+#define AT_THREADS 288
 #define AT_Q_BYTES (AT_BQ * 64 * 2)        // 16 KB
 #define AT_KV_BYTES (2 * AT_BK * 64 * 2)   // K tile 8 KB + V^T tile 8 KB per stage
-#define AT_P_BYTES (AT_BQ * AT_BK * 2)     // 16 KB per buffer
 
-__device__ __forceinline__ void at_ld32(uint32_t taddr, uint32_t (&v)[32]) { tc_ld32(taddr, v); }
 // 2^x on the SFU without the denormal fix-ups of exp2f (the arguments are <= 0; results below 2^-126 flush to zero and
 // round to zero in fp16 anyway)
 __device__ __forceinline__ float at_ex2(float x) {
@@ -47,44 +42,29 @@ __global__ void __launch_bounds__(AT_THREADS, 2)
 enc_attn_tc_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_k,
                    const __grid_constant__ CUtensorMap map_vt, __half* __restrict__ out, int S, int d) {
   extern __shared__ __align__(1024) unsigned char smem_raw[];
-  __shared__ __align__(8) uint64_t q_full, kv_full[AT_STAGES], kv_empty[AT_STAGES], s_full[2], p_full[2], d_full;
-  __shared__ uint32_t s_tmem_base;
-  __shared__ float s_mx[2][AT_BQ];      // [column half][row]: the two partial row sums, exchanged once at the end
+  __shared__ __align__(8) uint64_t q_full, kv_full[AT_STAGES], kv_empty[AT_STAGES];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int h = blockIdx.y, q0 = blockIdx.x * AT_BQ;
   const int nkb = (S + AT_BK - 1) / AT_BK;
-  const uint32_t smem_base = tc_smem_u32(smem_raw);
+  const uint32_t smem_base = (tc_smem_u32(smem_raw) + 1023u) & ~1023u;   // (1 KB of slack in the allocation)
   const uint32_t sQ = smem_base;
-  const uint32_t sKV = smem_base + AT_Q_BYTES;                           // stage s: K at +0, V^T at +8 KB
-  const uint32_t sP = smem_base + AT_Q_BYTES + AT_STAGES * AT_KV_BYTES;   // two P buffers
+  const uint32_t sKV = smem_base + AT_Q_BYTES;   // stage s: K at +0, V^T at +8 KB
 
-  if (warp == 0 && lane == 0) {
+  if (warp == 8 && lane == 0) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(&map_q) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&map_k) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&map_vt) : "memory");
     tc_mbar_init(tc_smem_u32(&q_full), 1);
-    for (int s = 0; s < AT_STAGES; ++s) { tc_mbar_init(tc_smem_u32(&kv_full[s]), 1); tc_mbar_init(tc_smem_u32(&kv_empty[s]), 1); }
-    for (int b = 0; b < 2; ++b) { tc_mbar_init(tc_smem_u32(&s_full[b]), 1); tc_mbar_init(tc_smem_u32(&p_full[b]), 8); }
-    tc_mbar_init(tc_smem_u32(&d_full), 1);
+    for (int s = 0; s < AT_STAGES; ++s) { tc_mbar_init(tc_smem_u32(&kv_full[s]), 1); tc_mbar_init(tc_smem_u32(&kv_empty[s]), 8); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tc_smem_u32(&s_tmem_base)),
-                 "n"(AT_TMEM_COLS)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = s_tmem_base;
-  const uint32_t tS0 = tmem_base, tD = tmem_base + 128;   // S buffers at columns 0 and 64, D at 128
   // programmatic dependent launch (tc_common.cuh): everything above overlapped the QKV GEMM's tail; Q, K and V^T are its
   // outputs
   tc_grid_dep_launch();
   tc_grid_dep_wait();
 
-  if (warp == 0) {
+  if (warp == 8) {
     // ===== TMA producer =====
     if (lane == 0) {
       tc_mbar_expect_tx(tc_smem_u32(&q_full), AT_Q_BYTES);
@@ -99,153 +79,96 @@ enc_attn_tc_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_const
         tc_tma_load_2d(sKV + s * AT_KV_BYTES + AT_BK * 64 * 2, &map_vt, kb * AT_BK, h * 64, full);
       }
     }
-  } else if (warp == 1) {
-    // ===== MMA issuer =====
-    if (lane == 0) {
-      const uint32_t idesc = tc_instr_desc_mn(128, 64);
-      const uint64_t qdesc = tc_smem_desc(sQ);
-      auto issue_qk = [&](int kb) {      // S_(kb & 1) = Q K(kb)^T
-        const int s = kb % AT_STAGES;
-        tc_mbar_wait(tc_smem_u32(&kv_full[s]), (kb / AT_STAGES) & 1);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const uint64_t kdesc = tc_smem_desc(sKV + s * AT_KV_BYTES);
+    return;
+  }
+
+  // ===== consumer warpgroup wg: query rows 64 wg .. 64 wg + 63 of the tile.  This thread holds rows r0 = 16 (warp % 4)
+  // + lane / 4 and r0 + 8, columns 8 j + 2 (lane % 4) + {0, 1} (j = 0..7) of the S and O fragments
+  const int wg = warp >> 2;
+  const int cq = 2 * (lane & 3);
+  const uint64_t qdesc = tc_smem_desc(sQ + wg * 64 * 128);
+  float o[32];
 #pragma unroll
-        for (int k = 0; k < 4; ++k)
-          tc_mma(tS0 + (uint32_t)((kb & 1) * 64), qdesc + (uint64_t)(k * 2), kdesc + (uint64_t)(k * 2), idesc, k > 0 ? 1u : 0u);
-        tc_commit(tc_smem_u32(&s_full[kb & 1]));
-      };
-      tc_mbar_wait(tc_smem_u32(&q_full), 0);
-      issue_qk(0);
-      if (nkb > 1) issue_qk(1);
-      for (int kb = 0; kb < nkb; ++kb) {
-        const int b = kb & 1, s = kb % AT_STAGES;
-        // P_b(kb) written, S_b(kb) and D(kb-1) read by the softmax warps
-        tc_mbar_wait(tc_smem_u32(&p_full[b]), (kb >> 1) & 1);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const uint64_t pdesc = tc_smem_desc(sP + b * AT_P_BYTES);
-        const uint64_t vdesc = tc_smem_desc(sKV + s * AT_KV_BYTES + AT_BK * 64 * 2);
+  for (int i = 0; i < 32; ++i) o[i] = 0.f;
+  float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
+  const float L2E = 1.4426950408889634f * 0.125f;   // log2(e) * head_dim^-0.5 (q is NOT pre-scaled)
+  tc_mbar_wait(tc_smem_u32(&q_full), 0);
+  for (int kb = 0; kb < nkb; ++kb) {
+    const int s = kb % AT_STAGES;
+    tc_mbar_wait(tc_smem_u32(&kv_full[s]), (kb / AT_STAGES) & 1);
+    const uint32_t sK = sKV + s * AT_KV_BYTES;
+    float sc[32];
 #pragma unroll
-        for (int k = 0; k < 4; ++k)
-          tc_mma(tD, pdesc + (uint64_t)(k * 2), vdesc + (uint64_t)(k * 2), idesc, k > 0 ? 1u : 0u);
-        tc_commit(tc_smem_u32(&kv_empty[s]));   // K(kb) (read by the earlier QK^T) and V^T(kb) are consumed
-        tc_commit(tc_smem_u32(&d_full));
-        if (kb + 2 < nkb) issue_qk(kb + 2);     // into S_b: its previous contents were read before p_full[b] fired
-      }
+    for (int i = 0; i < 32; ++i) sc[i] = 0.f;
+    wgmma_fence_regs(sc);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < 4; ++k) wgmma_ss_n64(sc, qdesc + (uint64_t)(k * 2), tc_smem_desc(sK) + (uint64_t)(k * 2), k > 0 ? 1u : 0u);
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_regs(sc);
+    const int nvalid = S - kb * AT_BK;   // existing keys of this block (only the last block is partial)
+    if (nvalid < AT_BK) {
+#pragma unroll
+      for (int j = 0; j < 8; ++j)
+#pragma unroll
+        for (int e = 0; e < 2; ++e)
+          if (8 * j + cq + e >= nvalid) { sc[4 * j + e] = -INFINITY; sc[4 * j + 2 + e] = -INFINITY; }
     }
-  } else {
-    // ===== softmax / output warps 2..9: TMEM lane quarter = warp % 4; TWO threads per query row, each owning 32 of the
-    // 64 key columns of a block (and 32 of the 64 output dims): the row maximum is exchanged through shared memory
-    const int qd = warp & 3;
-    const int hsel = (warp - 2) >> 2;            // 0: columns 0..31, 1: columns 32..63
-    const int rloc = qd * 32 + lane;             // row inside the tile (= TMEM lane)
-    const uint32_t lane_off = (uint32_t)(qd * 32) << 16;
-    float o[32];
+    uint32_t pa[4][4];   // P in the A-fragment layout of the four k16 steps of P V
 #pragma unroll
-    for (int i = 0; i < 32; ++i) o[i] = 0.f;
-    float m_run = -INFINITY, l_run = 0.f;
-    const float L2E = 1.4426950408889634f * 0.125f;   // log2(e) * head_dim^-0.5 (q is NOT pre-scaled)
-    for (int kb = 0; kb < nkb; ++kb) {
-      const int b = kb & 1;
-      tc_mbar_wait(tc_smem_u32(&s_full[b]), (kb >> 1) & 1);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      const int nvalid = S - kb * AT_BK - hsel * 32;   // existing keys among this thread's 32 columns
-      const bool full_block = nvalid >= 32;            // uniform per warp: only the last key block is partial
-      // row maximum over all 64 columns: the partner's half is read from TMEM too (cheaper than a shared-memory exchange
-      // and a 256-thread barrier per block); this thread's own half stays in registers for the exponentials
-      uint32_t sv[32];
+    for (int hr = 0; hr < 2; ++hr) {
       float mx = -INFINITY;
-      {
-        const int nv_o = S - kb * AT_BK - (hsel ^ 1) * 32;
-        at_ld32(tS0 + lane_off + (uint32_t)(b * 64 + (hsel ^ 1) * 32), sv);
-        if (nv_o >= 32) {
 #pragma unroll
-          for (int c = 0; c < 32; ++c) mx = fmaxf(mx, __uint_as_float(sv[c]));
-        } else {
-#pragma unroll
-          for (int c = 0; c < 32; ++c) mx = fmaxf(mx, (c < nv_o) ? __uint_as_float(sv[c]) : -INFINITY);
-        }
-      }
-      at_ld32(tS0 + lane_off + (uint32_t)(b * 64 + hsel * 32), sv);
-      if (full_block) {
-#pragma unroll
-        for (int c = 0; c < 32; ++c) mx = fmaxf(mx, __uint_as_float(sv[c]));
-      } else {
-#pragma unroll
-        for (int c = 0; c < 32; ++c) mx = fmaxf(mx, (c < nvalid) ? __uint_as_float(sv[c]) : -INFINITY);
-      }
-      const float m_new = fmaxf(m_run, mx);
-      const float alpha = at_ex2((m_run - m_new) * L2E);   // first block: 2^-inf = 0
+      for (int j = 0; j < 8; ++j) mx = fmaxf(mx, fmaxf(sc[4 * j + 2 * hr], sc[4 * j + 2 * hr + 1]));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+      const float m_new = fmaxf(m_run[hr], mx);
+      const float alpha = at_ex2((m_run[hr] - m_new) * L2E);   // first block: 2^-inf = 0
       const float msc = m_new * L2E;
-      m_run = m_new;
-      // P (fp16) into the K-major SWIZZLE_128B tile: row = rloc, 16-byte chunk c -> physical chunk c ^ (row & 7)
-      const uint32_t prow = sP + b * AT_P_BYTES + (uint32_t)rloc * 128u;
+      m_run[hr] = m_new;
       float lsum = 0.f;
 #pragma unroll
-      for (int c4 = 0; c4 < 4; ++c4) {
-        uint32_t pk[4];
-#pragma unroll
-        for (int e = 0; e < 4; ++e) {
-          const int c0 = c4 * 8 + 2 * e;
-          float p0 = at_ex2(fmaf(__uint_as_float(sv[c0]), L2E, -msc));
-          float p1 = at_ex2(fmaf(__uint_as_float(sv[c0 + 1]), L2E, -msc));
-          if (!full_block) {
-            if (c0 >= nvalid) p0 = 0.f;
-            if (c0 + 1 >= nvalid) p1 = 0.f;
-          }
-          lsum += p0 + p1;
-          pk[e] = pack_half2(p0, p1);
-        }
-        const int ch = hsel * 4 + c4;
-        asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(prow + (uint32_t)((ch ^ (rloc & 7)) << 4)), "r"(pk[0]),
-                     "r"(pk[1]), "r"(pk[2]), "r"(pk[3])
-                     : "memory");
+      for (int j = 0; j < 8; ++j) {
+        // masked keys: 2^-inf = 0
+        const float p0 = at_ex2(fmaf(sc[4 * j + 2 * hr], L2E, -msc));
+        const float p1 = at_ex2(fmaf(sc[4 * j + 2 * hr + 1], L2E, -msc));
+        lsum += p0 + p1;
+        pa[j >> 1][(j & 1) * 2 + hr] = pack_half2(p0, p1);
       }
-      l_run = fmaf(l_run, alpha, lsum);
-      // O (this thread's 32 dims): add the previous block's P V, then rescale to the new running maximum
-      if (kb > 0) {
-        tc_mbar_wait(tc_smem_u32(&d_full), (kb - 1) & 1);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        uint32_t dv[32];
-        at_ld32(tD + lane_off + (uint32_t)(hsel * 32), dv);
-#pragma unroll
-        for (int c = 0; c < 32; ++c) o[c] += __uint_as_float(dv[c]);
-      }
+      l_run[hr] = fmaf(l_run[hr], alpha, lsum);
       if (alpha != 1.0f) {   // the running maximum rarely moves after the first blocks
 #pragma unroll
-        for (int c = 0; c < 32; ++c) o[c] *= alpha;
+        for (int j = 0; j < 8; ++j) { o[4 * j + 2 * hr] *= alpha; o[4 * j + 2 * hr + 1] *= alpha; }
       }
-      // P_b visible to the tensor core (async proxy), S_b and D free for the next products
-      asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-      __syncwarp();
-      if (lane == 0) asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(tc_smem_u32(&p_full[b])) : "memory");
     }
-    tc_mbar_wait(tc_smem_u32(&d_full), (nkb - 1) & 1);
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    {
-      uint32_t dv[32];
-      at_ld32(tD + lane_off + (uint32_t)(hsel * 32), dv);
+    const uint64_t vdesc = tc_smem_desc(sK + AT_BK * 64 * 2);
+    wgmma_fence_regs(o);
+    wgmma_fence();
 #pragma unroll
-      for (int c = 0; c < 32; ++c) o[c] += __uint_as_float(dv[c]);
-    }
-    // the two halves of a row used the same running maxima: their sums add up
-    s_mx[hsel][rloc] = l_run;
-    asm volatile("bar.sync 1, 256;" ::: "memory");
-    l_run += s_mx[hsel ^ 1][rloc];
-    const int row = q0 + rloc;
-    if (row < S) {
-      const float inv = 1.0f / l_run;
-      uint4* dst = reinterpret_cast<uint4*>(out + (size_t)row * d + h * 64 + hsel * 32);
-#pragma unroll
-      for (int ch = 0; ch < 4; ++ch)
-        dst[ch] = make_uint4(pack_half2(o[ch * 8 + 0] * inv, o[ch * 8 + 1] * inv), pack_half2(o[ch * 8 + 2] * inv, o[ch * 8 + 3] * inv),
-                             pack_half2(o[ch * 8 + 4] * inv, o[ch * 8 + 5] * inv), pack_half2(o[ch * 8 + 6] * inv, o[ch * 8 + 7] * inv));
-    }
+    for (int k = 0; k < 4; ++k) wgmma_rs_n64(o, pa[k], vdesc + (uint64_t)(k * 2), 1u);
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_regs(o);
+    __syncwarp();
+    if (lane == 0) tc_mbar_arrive(tc_smem_u32(&kv_empty[s]));   // K(kb) and V^T(kb) are consumed
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 1) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(AT_TMEM_COLS) : "memory");
+  // the four threads of a quad summed disjoint columns with the same running maxima: their sums add up
+#pragma unroll
+  for (int hr = 0; hr < 2; ++hr) {
+    l_run[hr] += __shfl_xor_sync(0xffffffffu, l_run[hr], 1);
+    l_run[hr] += __shfl_xor_sync(0xffffffffu, l_run[hr], 2);
+  }
+#pragma unroll
+  for (int hr = 0; hr < 2; ++hr) {
+    const int row = q0 + wg * 64 + (warp & 3) * 16 + (lane >> 2) + hr * 8;
+    if (row < S) {
+      const float inv = 1.0f / l_run[hr];
+      __half* dst = out + (size_t)row * d + h * 64 + cq;
+#pragma unroll
+      for (int j = 0; j < 8; ++j)
+        *reinterpret_cast<uint32_t*>(dst + 8 * j) = pack_half2(o[4 * j + 2 * hr] * inv, o[4 * j + 2 * hr + 1] * inv);
+    }
   }
 }
 
@@ -295,7 +218,7 @@ static bool at_make_map(CUtensorMap* map, const __half* base, uint64_t rows, uin
             CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
-static const size_t kAtSmem = (size_t)AT_Q_BYTES + (size_t)AT_STAGES * AT_KV_BYTES + 2 * AT_P_BYTES + 1024;
+static const size_t kAtSmem = (size_t)AT_Q_BYTES + (size_t)AT_STAGES * AT_KV_BYTES + 1024;
 
 cudaError_t enc_attention_tc_configure() {
   cudaError_t e = cudaFuncSetAttribute(enc_attn_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kAtSmem);

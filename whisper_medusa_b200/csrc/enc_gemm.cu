@@ -4,8 +4,8 @@
 // and the cross-attention K/V projection of every decoder layer (:325-336).
 //
 // This file is the mma.sync (m16n8k16) implementation: 128x128x32 CTA tile, 8 warps (2x4), 4-stage
-// cp.async pipeline, XOR-swizzled shared memory read with ldmatrix.  The tcgen05/TMA version in
-// enc_gemm_tc.cu replaces it on the hot path once validated against it.
+// cp.async pipeline, XOR-swizzled shared memory read with ldmatrix.  The wgmma/TMA version in
+// enc_gemm_tc.cu replaces it on the hot path; this one is its cross-check.
 #include "common.cuh"
 #include "engine.h"
 #include "tc_common.cuh"

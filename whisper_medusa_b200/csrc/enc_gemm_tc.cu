@@ -1,22 +1,17 @@
-// Encoder-side dense GEMM on the 5th-generation tensor cores (sm_100a):
-//   C[M,N] = A[M,K] * W[N,K]^T   fp16 operands (both K-major), fp32 accumulation in TMEM.
+// Encoder-side dense GEMM on the Hopper tensor cores (sm_90a, wgmma):
+//   C[M,N] = A[M,K] * W[N,K]^T   fp16 operands (both K-major), fp32 accumulation in registers.
 //
-// Structure: one (128 MB) x BN output tile per CTA, K swept in 64-column blocks.  At M = 1500 these GEMMs are bound by
-// the rate at which ONE SM can pull operands out of L2 (about 80 GB/s per SM, measured), not by the tensor pipe: a tile
-// costs (BM + BN) * K * 2 bytes, so the host picks, per GEMM, the tile shape with the fewest operand bytes on the
-// busiest SM (see pick_tile and DESIGN.md):
-//   MB = 1, BN = 128 (or 64), 3-stage ring, two CTAs per SM (one tile's epilogue overlaps the other's main loop);
-//   MB = 1, BN = 128, 6-stage ring, one CTA per SM: outputs too narrow to give every SM two tiles;
-//   MB = 2, BN = 128 / 192 / 256, one CTA per SM: two 128-row accumulators share every W tile (up to all 512 TMEM
-//   columns) -- wide outputs in ONE wave of <= 148 tiles.
-//   warp 0  : TMA producer   -- cp.async.bulk.tensor.2d (SWIZZLE_128B) of the A and W tiles into a
-//                               shared-memory ring, completion on `full` mbarriers
-//   warp 1  : MMA issuer     -- one elected thread issues tcgen05.mma.cta_group::1.kind::f16
-//                               (M=128, N=BN, K=16) x4 (x MB) per stage, accumulators = MB * BN TMEM columns;
-//                               tcgen05.commit releases the stage (`empty`) / signals the epilogue
-//   warps 2.. : epilogue     -- 2 (MB = 1) or 4 (MB = 2) warps per TMEM lane quarter, 32-column blocks dealt round-robin: tcgen05.ld
-//                               (32 lanes x 32 columns per instruction) -> registers ->
-//                               bias / GELU / residual / position epilogue -> global
+// Structure: one BM x BN output tile per CTA, K swept in 64-column blocks.  At M = 1500 a GEMM has few tiles per SM,
+// so the host picks, per GEMM, the tile shape with the fewest operand bytes on the busiest SM (see pick_tile):
+//   128 x 128, 6-stage ring, one CTA per SM: outputs of <= 1536 columns and the fp32 read-modify-write epilogues;
+//   128 x 128, 3-stage ring, two CTAs per SM (one tile's epilogue overlaps the other's main loop): other narrow tiles;
+//   256 x 128, 128 x 192, 128 x 256: wide fp16 outputs, one CTA per SM, fewer rounds of tiles over the SMs.
+//   warp 8    : TMA producer -- cp.async.bulk.tensor.2d (SWIZZLE_128B) of the A and W tiles into a shared-memory ring,
+//                               completion on `full` mbarriers
+//   warps 0-7 : two consumer warpgroups, each owning BM / 2 rows of the tile: wgmma.mma_async m64nBNk16 (A and W from
+//               shared memory) x4 per stage and 64-row slice, one wgmma group kept in flight; a stage is released
+//               (`empty`) once the group that read it has completed.  Epilogue: accumulators + bias -> the idle ring as
+//               an fp32 tile -> GELU / residual / positions applied while the tile is copied out row-contiguously.
 // The A operand may be an "implicit im2col" view: conv1/conv2 read a time-major activation whose
 // GEMM rows overlap (row stride 80 resp. 2d elements) -- the TMA tensor map simply carries that
 // stride, no im2col buffer exists.
@@ -35,23 +30,9 @@ namespace wm {
 #define TC_BM 128
 #define TC_BN 128
 #define TC_BK 64
-#ifndef WM_TC_NARROW_BN
-#define WM_TC_NARROW_BN 128   /* tile width for outputs of <= 1536 columns (64: twice the tiles, 3 stages, 2 CTAs / SM) */
-#endif
-#ifndef WM_TC_W192_STAGES
-#define WM_TC_W192_STAGES 4   /* ring depth of the 256 x 192 tiles (225 KB; 3 stages: 5.54 vs 5.51 ms per clip) */
-#endif
-#ifndef WM_TC_SMEM_BIAS
-#define WM_TC_SMEM_BIAS 1     /* 0: bias values read from global memory inside the epilogue (A/B) */
-#endif
-#define TC_THREADS 320       /* MB = 1: TMA warp + MMA warp + 8 epilogue warps */
-#define TC_THREADS_WIDE 576  /* MB = 2: ... + 16 epilogue warps (the epilogue of the single wave is exposed) */
-__host__ __device__ constexpr int tc_stage_bytes(int mb, int bn) {
-  return mb == 1 ? (TC_BM + TC_BN) * TC_BK * 2 /* any width: A at 0, W at 16 KB */ : (mb * TC_BM + bn) * TC_BK * 2;
-}
-__host__ __device__ constexpr int tc_tmem_cols(int mb, int bn) {
-  return mb * bn <= 128 ? 128 : (mb * bn <= 256 ? 256 : 512);
-}
+#define TC_THREADS 288   /* two consumer warpgroups + one TMA warp */
+__host__ __device__ constexpr int tc_stage_bytes(int bm, int bn) { return (bm + bn) * TC_BK * 2; }
+__host__ __device__ constexpr int tc_stage_ld(int bn) { return bn + 8; }   // fp32 epilogue tile row stride (floats)
 
 struct TcArgs {
   int M, N, K;
@@ -64,47 +45,46 @@ struct TcArgs {
   __half* ck; __half* cv; int kv_spad;   // non-null: the output [pos][k | v] goes to the decode layout [head][kv_spad][72]
 };
 
-template <int EPI, int MB, int BN, int STAGES>
-__global__ void __launch_bounds__(MB == 1 ? TC_THREADS : TC_THREADS_WIDE, MB == 1 ? 2 : 1)
+template <int BN>
+__device__ __forceinline__ void tc_wgmma(float (&d)[BN / 2], uint64_t adesc, uint64_t bdesc, uint32_t acc) {
+  if constexpr (BN == 64) wgmma_ss_n64(d, adesc, bdesc, acc);
+  else if constexpr (BN == 128) wgmma_ss_n128(d, adesc, bdesc, acc);
+  else if constexpr (BN == 192) wgmma_ss_n192(d, adesc, bdesc, acc);
+  else wgmma_ss_n256(d, adesc, bdesc, acc);
+}
+
+template <int EPI, int BM, int BN, int STAGES>
+__global__ void __launch_bounds__(TC_THREADS, (BM == 128 && BN == 128 && STAGES == 3) ? 2 : 1)
 enc_gemm_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_w, TcArgs a) {
   extern __shared__ __align__(1024) unsigned char smem_raw[];
-  // stage s: A tile [128 MB rows][64 halfs] at s * STAGE_BYTES, W tile [BN rows][64 halfs] behind it (both 1024-B
-  // aligned, SW128)
-  constexpr int STAGE_BYTES = tc_stage_bytes(MB, BN);
-  constexpr int A_BYTES = MB * TC_BM * TC_BK * 2;
-  constexpr int TMEM_COLS = tc_tmem_cols(MB, BN);
-  constexpr int NEPI_Q = (MB == 1 ? TC_THREADS / 32 - 2 : TC_THREADS_WIDE / 32 - 2) / 4;   // epilogue warps per lane quarter
-  __shared__ __align__(8) uint64_t s_full[STAGES], s_empty[STAGES], s_tmem_full;
-  __shared__ uint32_t s_tmem_base;
+  // stage s: A tile [BM rows][64 halfs] at s * STAGE_BYTES, W tile [BN rows][64 halfs] behind it (both 1024-B aligned, SW128)
+  constexpr int STAGE_BYTES = tc_stage_bytes(BM, BN);
+  constexpr int A_BYTES = BM * TC_BK * 2;
+  constexpr int MI = BM / 128;            // 64-row slices per consumer warpgroup
+  constexpr int LD = tc_stage_ld(BN);
+  static_assert(BM * LD * 4 <= STAGES * STAGE_BYTES, "the fp32 epilogue tile must fit in the ring");
+  __shared__ __align__(8) uint64_t s_full[STAGES], s_empty[STAGES];
   __shared__ __align__(16) float s_bias[BN];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int m0 = blockIdx.y * (MB * TC_BM), n0 = blockIdx.x * BN;
+  const int m0 = blockIdx.y * BM, n0 = blockIdx.x * BN;
   const int KT = a.K / TC_BK;
-  const uint32_t smem_base = tc_smem_u32(smem_raw);
+  // 1024-B aligned base (the dynamic allocation carries 1 KB of slack)
+  const uint32_t smem_base = (tc_smem_u32(smem_raw) + 1023u) & ~1023u;
+  unsigned char* const smem = smem_raw + (smem_base - tc_smem_u32(smem_raw));
 
-  if (warp == 0 && lane == 0) {
+  if (warp == 8 && lane == 0) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(&map_a) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&map_w) : "memory");
     for (int s = 0; s < STAGES; ++s) {
       tc_mbar_init(tc_smem_u32(&s_full[s]), 1);
-      tc_mbar_init(tc_smem_u32(&s_empty[s]), 1);
+      tc_mbar_init(tc_smem_u32(&s_empty[s]), 8);   // lane 0 of every consumer warp
     }
-    tc_mbar_init(tc_smem_u32(&s_tmem_full), 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tc_smem_u32(&s_tmem_base)),
-                 "n"(TMEM_COLS)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = s_tmem_base;
   tc_grid_dep_launch();
 
-  if (warp == 0) {
+  if (warp == 8) {
     // ===== TMA producer =====
     if (lane == 0) {
       // the weight tiles of the first ring round do not depend on the predecessor kernel: they are requested before the
@@ -112,146 +92,129 @@ enc_gemm_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_const
       const int pre = KT < STAGES ? KT : STAGES;
       for (int kt = 0; kt < pre; ++kt) {
         const uint32_t full = tc_smem_u32(&s_full[kt]);
-        tc_mbar_expect_tx(full, (MB * TC_BM + BN) * TC_BK * 2);
+        tc_mbar_expect_tx(full, STAGE_BYTES);
         tc_tma_load_2d(smem_base + kt * STAGE_BYTES + A_BYTES, &map_w, kt * TC_BK, n0, full);
       }
       tc_grid_dep_wait();
       for (int kt = 0; kt < pre; ++kt)
-        tc_tma_load_2d(smem_base + kt * STAGE_BYTES, &map_a, kt * TC_BK, m0, tc_smem_u32(&s_full[kt]));   // (one box of 128 MB rows)
+        tc_tma_load_2d(smem_base + kt * STAGE_BYTES, &map_a, kt * TC_BK, m0, tc_smem_u32(&s_full[kt]));
       for (int kt = pre; kt < KT; ++kt) {
         const int s = kt % STAGES;
         const uint32_t ph = (kt / STAGES) & 1;
         tc_mbar_wait(tc_smem_u32(&s_empty[s]), ph ^ 1);
         const uint32_t full = tc_smem_u32(&s_full[s]);
-        tc_mbar_expect_tx(full, (MB * TC_BM + BN) * TC_BK * 2);
+        tc_mbar_expect_tx(full, STAGE_BYTES);
         tc_tma_load_2d(smem_base + s * STAGE_BYTES, &map_a, kt * TC_BK, m0, full);
         tc_tma_load_2d(smem_base + s * STAGE_BYTES + A_BYTES, &map_w, kt * TC_BK, n0, full);
       }
     }
-  } else if (warp == 1) {
-    // ===== MMA issuer =====
-    if (lane == 0) {
-      const uint32_t idesc = tc_instr_desc(BN);
-      for (int kt = 0; kt < KT; ++kt) {
-        const int s = kt % STAGES;
-        const uint32_t ph = (kt / STAGES) & 1;
-        tc_mbar_wait(tc_smem_u32(&s_full[s]), ph);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const uint64_t adesc = tc_smem_desc(smem_base + s * STAGE_BYTES);
-        const uint64_t bdesc = tc_smem_desc(smem_base + s * STAGE_BYTES + A_BYTES);
+    return;
+  }
+
+  // ===== consumer warpgroups =====
+  const int wg = warp >> 2;                  // rows [wg * BM / 2, (wg + 1) * BM / 2) of the tile
+  const int tid = threadIdx.x;               // 0 .. 255
+  for (int i = tid; i < BN; i += 256) s_bias[i] = a.bias[n0 + i];
+  float acc[MI][BN / 2];
 #pragma unroll
-        for (int k = 0; k < TC_BK / 16; ++k) {
-          // advance 16 halfs = 32 B inside the 128-B swizzle atom: +2 in the (>>4) start address; the second 128-row
-          // block of A lies 16 KB further, its accumulator BN columns further
+  for (int i = 0; i < MI; ++i)
 #pragma unroll
-          for (int mb = 0; mb < MB; ++mb)
-            tc_mma(tmem_base + (uint32_t)(mb * BN), adesc + (uint64_t)(mb * ((TC_BM * TC_BK * 2) >> 4) + k * 2),
-                   bdesc + (uint64_t)(k * 2), idesc, (kt > 0 || k > 0) ? 1u : 0u);
+    for (int j = 0; j < BN / 2; ++j) acc[i][j] = 0.f;
+  for (int kt = 0; kt < KT; ++kt) {
+    const int s = kt % STAGES;
+    tc_mbar_wait(tc_smem_u32(&s_full[s]), (kt / STAGES) & 1);
+    const uint64_t adesc = tc_smem_desc(smem_base + s * STAGE_BYTES + wg * (BM / 2) * 128);
+    const uint64_t bdesc = tc_smem_desc(smem_base + s * STAGE_BYTES + A_BYTES);
+#pragma unroll
+    for (int i = 0; i < MI; ++i) wgmma_fence_regs(acc[i]);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < TC_BK / 16; ++k)
+#pragma unroll
+      for (int i = 0; i < MI; ++i)
+        tc_wgmma<BN>(acc[i], adesc + (uint64_t)(i * 512 + k * 2), bdesc + (uint64_t)(k * 2), (kt > 0 || k > 0) ? 1u : 0u);
+    wgmma_commit();
+    wgmma_wait<1>();   // the group of stage kt - 1 has completed: its ring slot may be refilled
+#pragma unroll
+    for (int i = 0; i < MI; ++i) wgmma_fence_regs(acc[i]);
+    if (kt > 0 && lane == 0) tc_mbar_arrive(tc_smem_u32(&s_empty[(kt - 1) % STAGES]));
+  }
+  wgmma_wait<0>();
+#pragma unroll
+  for (int i = 0; i < MI; ++i) wgmma_fence_regs(acc[i]);
+  tc_grid_dep_wait();   // (the epilogue reads and writes activations)
+  // every consumer is done with the ring (and s_bias is complete): the ring becomes the fp32 tile [BM][LD]
+  asm volatile("bar.sync 1, 256;" ::: "memory");
+  float* const tile = reinterpret_cast<float*>(smem);
+  {
+    const int r_w = wg * (BM / 2) + (warp & 3) * 16 + (lane >> 2), c_q = 2 * (lane & 3);
+#pragma unroll
+    for (int i = 0; i < MI; ++i)
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j)
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int r = r_w + i * 64 + h * 8, c = j * 8 + c_q;
+          *reinterpret_cast<float2*>(tile + r * LD + c) =
+              make_float2(acc[i][4 * j + 2 * h] + s_bias[c], acc[i][4 * j + 2 * h + 1] + s_bias[c + 1]);
         }
-        tc_commit(tc_smem_u32(&s_empty[s]));      // stage reusable once these MMAs have read it
+  }
+  asm volatile("bar.sync 1, 256;" ::: "memory");
+  constexpr bool F32_OUT = (EPI == ENC_EPI_BIAS_RES_F32 || EPI == ENC_EPI_BIAS_GELU_POS_F32);
+  if constexpr (!F32_OUT) {
+    // 8 consecutive columns of one row per thread: one 16-byte store
+    for (int it = tid; it < BM * (BN / 8); it += 256) {
+      const int r = it / (BN / 8), c = (it % (BN / 8)) * 8;
+      const int row = m0 + r, col = n0 + c;
+      if (row >= a.M) continue;
+      const float4 x0 = *reinterpret_cast<const float4*>(tile + r * LD + c);
+      const float4 x1 = *reinterpret_cast<const float4*>(tile + r * LD + c + 4);
+      float x[8] = {x0.x, x0.y, x0.z, x0.w, x1.x, x1.y, x1.z, x1.w};
+      if (EPI == ENC_EPI_BIAS_GELU_F16) {
+#pragma unroll
+        for (int e = 0; e < 8; ++e) x[e] = gelu_erf(x[e]);
       }
-      tc_commit(tc_smem_u32(&s_tmem_full));       // accumulator complete
+      __half* dst = a.out16 + (size_t)row * a.ldo16 + col;
+      if (EPI == ENC_EPI_BIAS_F16 && a.ck != nullptr) {
+        // cross-attention K/V straight into the layout the decode kernels read: [head][position][64 dims + 8 pad]
+        // (pad halfs and positions >= M stay zero from the allocation)
+        const int dm = a.N >> 1;
+        const int cc = col >= dm ? col - dm : col;
+        dst = (col >= dm ? a.cv : a.ck) + ((size_t)(cc >> 6) * a.kv_spad + row) * 72 + (cc & 63);
+      }
+      *reinterpret_cast<uint4*>(dst) = make_uint4(pack_half2(x[0], x[1]), pack_half2(x[2], x[3]), pack_half2(x[4], x[5]),
+                                                  pack_half2(x[6], x[7]));
+    }
+    if (EPI == ENC_EPI_BIAS_F16 && a.vt != nullptr && n0 + BN > a.vt_col0) {
+      // V^T for the attention kernel: two consecutive positions of one column per thread, so a warp writes 128
+      // contiguous bytes of a V^T row
+      for (int it = tid; it < BN * (BM / 2); it += 256) {
+        const int c = it / (BM / 2), r = (it % (BM / 2)) * 2;
+        const int row = m0 + r, col = n0 + c;
+        if (col < a.vt_col0 || row >= a.M) continue;
+        __half* vdst = a.vt + (size_t)(col - a.vt_col0) * a.vt_ld + row;
+        const __half2 hh = __floats2half2_rn(tile[r * LD + c], tile[(r + 1) * LD + c]);
+        if (row + 1 < a.M) *reinterpret_cast<__half2*>(vdst) = hh;
+        else vdst[0] = __low2half(hh);
+      }
     }
   } else {
-    // ===== epilogue: a warp reads the TMEM lane quarter (warp % 4) =====
-    // The bias row of the tile goes to shared memory while the main loop runs (these warps idle until the accumulator
-    // is complete).  (A/B, rejected: also pulling the residual / position values of the fp32 epilogues into registers
-    // before the accumulator is complete -- 64 more live registers, 5.75 vs 5.54 ms per clip.)
-    const int q = warp & 3;
-    constexpr int NEPI_T = NEPI_Q * 4 * 32;
-    constexpr int NBLK = MB * (BN / 32) / NEPI_Q;   // 32 x 32 blocks per warp
-    constexpr bool F32_OUT = (EPI == ENC_EPI_BIAS_RES_F32 || EPI == ENC_EPI_BIAS_GELU_POS_F32);
-    for (int i = (int)threadIdx.x - 64; i < BN; i += NEPI_T) s_bias[i] = a.bias[n0 + i];
-    tc_grid_dep_wait();   // (the epilogue reads and writes activations)
-    asm volatile("bar.sync 1, %0;" ::"n"(NEPI_T) : "memory");   // (epilogue warps only) s_bias complete
-    tc_mbar_wait(tc_smem_u32(&s_tmem_full), 0);
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    auto block = [&](const int blk) {
-      const int mb = blk / (BN / 32), cb = blk % (BN / 32);
-      const int row = m0 + mb * TC_BM + q * 32 + lane;
-      const bool row_ok = row < a.M;
-      uint32_t v[32];
-      tc_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(mb * BN + cb * 32), v);
-      const int col0 = n0 + cb * 32;
-      if constexpr (!F32_OUT) {
-        if (!row_ok) return;
-        __half* dst = a.out16 + (size_t)row * a.ldo16 + col0;
-        if (EPI == ENC_EPI_BIAS_F16 && a.ck != nullptr) {
-          // cross-attention K/V straight into the layout the decode kernels read: [head][position][64 dims + 8 pad]
-          // (pad halfs and positions >= M stay zero from the allocation); 64 contiguous bytes per thread as above
-          const int dm = a.N >> 1;
-          const int cc = col0 >= dm ? col0 - dm : col0;
-          dst = (col0 >= dm ? a.cv : a.ck) + ((size_t)(cc >> 6) * a.kv_spad + row) * 72 + (cc & 63);
-        }
-#pragma unroll
-        for (int c8 = 0; c8 < 4; ++c8) {
-          const float* bsrc = WM_TC_SMEM_BIAS ? &s_bias[cb * 32 + c8 * 8] : a.bias + col0 + c8 * 8;
-          const float4 b0 = *reinterpret_cast<const float4*>(bsrc);
-          const float4 b1 = *reinterpret_cast<const float4*>(bsrc + 4);
-          const float bb[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
-          uint32_t pk[4];
-#pragma unroll
-          for (int e = 0; e < 4; ++e) {
-            float x0 = __uint_as_float(v[c8 * 8 + 2 * e]) + bb[2 * e];
-            float x1 = __uint_as_float(v[c8 * 8 + 2 * e + 1]) + bb[2 * e + 1];
-            if (EPI == ENC_EPI_BIAS_GELU_F16) { x0 = gelu_erf(x0); x1 = gelu_erf(x1); }
-            pk[e] = pack_half2(x0, x1);
-          }
-          *reinterpret_cast<uint4*>(dst + c8 * 8) = make_uint4(pk[0], pk[1], pk[2], pk[3]);
-          if (EPI == ENC_EPI_BIAS_F16 && a.vt != nullptr && col0 >= a.vt_col0) {
-            // V^T for the tcgen05 attention: thread = position, so for a fixed column the 32 lanes write 32
-            // consecutive halfs (64 contiguous bytes)
-            __half* vcol = a.vt + (size_t)(col0 - a.vt_col0 + c8 * 8) * a.vt_ld + row;
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-              const __half2 hh = *reinterpret_cast<const __half2*>(&pk[e]);
-              vcol[(size_t)(2 * e) * a.vt_ld] = __low2half(hh);
-              vcol[(size_t)(2 * e + 1) * a.vt_ld] = __high2half(hh);
-            }
-          }
-        }
+    // fp32 read-modify-write epilogues (residual stream / conv2 + positions): 4 consecutive columns per thread
+    for (int it = tid; it < BM * (BN / 4); it += 256) {
+      const int r = it / (BN / 4), c = (it % (BN / 4)) * 4;
+      const int row = m0 + r, col = n0 + c;
+      if (row >= a.M) continue;
+      const float4 x = *reinterpret_cast<const float4*>(tile + r * LD + c);
+      float* dst = a.out32 + (size_t)row * a.ldo32 + col;
+      if (EPI == ENC_EPI_BIAS_RES_F32) {
+        const float4 in = *reinterpret_cast<const float4*>(dst);
+        *reinterpret_cast<float4*>(dst) = make_float4(in.x + x.x, in.y + x.y, in.z + x.z, in.w + x.w);
       } else {
-        // fp32 read-modify-write epilogues (residual stream / conv2 + positions).  tcgen05.ld hands every thread one ROW
-        // of the tile; row-wise global accesses would touch 32 different lines per instruction (the kernel then spends
-        // most of its time waiting for the residual loads -- ncu, round 2).  The 32 x 32 block is transposed through
-        // shared memory (the pipeline stages are idle once the accumulator is complete): lane = column, so every
-        // load / store of the residual stream is one contiguous 128-byte segment.
-        float* sC = reinterpret_cast<float*>(smem_raw) + (size_t)(warp - 2) * (32 * 33);
-        __syncwarp();
-#pragma unroll
-        for (int c = 0; c < 32; ++c) sC[lane * 33 + c] = __uint_as_float(v[c]);
-        __syncwarp();
-        const float bcol = WM_TC_SMEM_BIAS ? s_bias[cb * 32 + lane] : a.bias[col0 + lane];
-        const int row_base = m0 + mb * TC_BM + q * 32;
-#pragma unroll 1
-        for (int r0 = 0; r0 < 32; r0 += 8) {
-          float in[8];
-#pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            const int rr = row_base + r0 + i;
-            in[i] = 0.f;
-            if (rr < a.M)
-              in[i] = (EPI == ENC_EPI_BIAS_RES_F32) ? a.out32[(size_t)rr * a.ldo32 + col0 + lane]
-                                                    : a.pos[(size_t)rr * a.N + col0 + lane];
-          }
-#pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            const int rr = row_base + r0 + i;
-            if (rr < a.M) {
-              const float x = sC[(r0 + i) * 33 + lane] + bcol;
-              a.out32[(size_t)rr * a.ldo32 + col0 + lane] = (EPI == ENC_EPI_BIAS_RES_F32) ? in[i] + x : gelu_erf(x) + in[i];
-            }
-          }
-        }
+        const float4 in = *reinterpret_cast<const float4*>(a.pos + (size_t)row * a.N + col);
+        *reinterpret_cast<float4*>(dst) =
+            make_float4(gelu_erf(x.x) + in.x, gelu_erf(x.y) + in.y, gelu_erf(x.z) + in.z, gelu_erf(x.w) + in.w);
       }
-    };
-#pragma unroll 1
-    for (int b = 0; b < NBLK; ++b) block(((warp - 2) >> 2) + b * NEPI_Q);
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 1) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(TMEM_COLS) : "memory");
+    }
   }
 }
 
@@ -288,11 +251,11 @@ static bool make_map(CUtensorMap* map, const __half* base, uint64_t rows, uint64
   return r == CUDA_SUCCESS;
 }
 
-static constexpr size_t tc_smem(int mb, int bn, int stages) { return (size_t)stages * tc_stage_bytes(mb, bn) + 1024; }
+static constexpr size_t tc_smem(int bm, int bn, int stages) { return (size_t)stages * tc_stage_bytes(bm, bn) + 1024; }
 
-// every instantiation: X(EPI, MB, BN, STAGES)
-#define WM_TC_NARROW_TILES(X, EPI) X(EPI, 1, 128, 3) X(EPI, 1, 128, 6) X(EPI, 1, 64, 3)
-#define WM_TC_WIDE_TILES(X, EPI) X(EPI, 2, 128, 4) X(EPI, 2, 192, WM_TC_W192_STAGES) X(EPI, 2, 256, 3)
+// every instantiation: X(EPI, BM, BN, STAGES)
+#define WM_TC_NARROW_TILES(X, EPI) X(EPI, 128, 128, 3) X(EPI, 128, 128, 6)
+#define WM_TC_WIDE_TILES(X, EPI) X(EPI, 256, 128, 4) X(EPI, 128, 192, 5) X(EPI, 128, 256, 4)
 #define WM_TC_ALL(X)                                                                                             \
   WM_TC_NARROW_TILES(X, ENC_EPI_BIAS_F16) WM_TC_NARROW_TILES(X, ENC_EPI_BIAS_GELU_F16)                           \
   WM_TC_NARROW_TILES(X, ENC_EPI_BIAS_RES_F32) WM_TC_NARROW_TILES(X, ENC_EPI_BIAS_GELU_POS_F32)                   \
@@ -300,34 +263,33 @@ static constexpr size_t tc_smem(int mb, int bn, int stages) { return (size_t)sta
 
 cudaError_t enc_gemm_tc_configure() {
   cudaError_t e;
-#define WM_SET(EPI, MB, BN, ST)                                                                                          \
-  e = cudaFuncSetAttribute(enc_gemm_tc_kernel<EPI, MB, BN, ST>, cudaFuncAttributeMaxDynamicSharedMemorySize,             \
-                           (int)tc_smem(MB, BN, ST));                                                                    \
+#define WM_SET(EPI, BM, BN, ST)                                                                                          \
+  e = cudaFuncSetAttribute(enc_gemm_tc_kernel<EPI, BM, BN, ST>, cudaFuncAttributeMaxDynamicSharedMemorySize,             \
+                           (int)tc_smem(BM, BN, ST));                                                                    \
   if (e != cudaSuccess) return e;
   WM_TC_ALL(WM_SET)
 #undef WM_SET
   return get_encode_fn() ? cudaSuccess : cudaErrorNotSupported;
 }
 
-// Tile shape of one GEMM.  The operand bytes the busiest SM pulls out of L2 decide the time: tiles are dealt to the
-// 148 SMs in ceil(tiles / 148) rounds of K * (BM + BN) * 2 bytes each.  Candidates with two 128-row blocks per CTA exist
-// for the fp16-output epilogues only (the fp32 read-modify-write epilogues feed N = d outputs: too few tiles already).
-struct TcTile { int mb, bn, stages; };
+// Tile shape of one GEMM.  Tiles are dealt to the SMs in ceil(tiles / n_sm) rounds of K * (BM + BN) * 2 operand bytes
+// each; the shape with the fewest operand bytes on the busiest SM wins.  The wide candidates exist for the fp16-output
+// epilogues only (the fp32 read-modify-write epilogues feed N = d outputs: too few tiles already).
+struct TcTile { int bm, bn, stages; };
 static TcTile pick_tile(const EncGemmArgs& g, int n_sm) {
-  const bool narrow = g.N <= 1536;   // fewer than one 128 x 128 tile per SM and round
-  TcTile best = {1, (narrow && WM_TC_NARROW_BN == 64 && g.N % 64 == 0) ? 64 : TC_BN, 3};
-  if (narrow && best.bn == TC_BN) best.stages = 6;
+  const bool narrow = g.N <= 1536;   // few 128 x 128 tiles per SM and round: one CTA per SM with a deep ring
+  TcTile best = {TC_BM, TC_BN, narrow ? 6 : 3};
   const bool f16_out = g.epi == ENC_EPI_BIAS_F16 || g.epi == ENC_EPI_BIAS_GELU_F16;
   if (g.tile == 1 || !f16_out) return best;
-  auto cost = [&](int mb, int bn) {
-    const long tiles = (long)((g.M + mb * TC_BM - 1) / (mb * TC_BM)) * (g.N / bn);
-    return ((tiles + n_sm - 1) / n_sm) * (long)(mb * TC_BM + bn);
+  auto cost = [&](int bm, int bn) {
+    const long tiles = (long)((g.M + bm - 1) / bm) * (g.N / bn);
+    return ((tiles + n_sm - 1) / n_sm) * (long)(bm + bn);
   };
-  long c = cost(1, best.bn);
-  const TcTile wide[3] = {{2, 128, 4}, {2, 192, WM_TC_W192_STAGES}, {2, 256, 3}};
+  long c = cost(best.bm, best.bn);
+  const TcTile wide[3] = {{256, 128, 4}, {128, 192, 5}, {128, 256, 4}};
   for (const TcTile& t : wide) {
     if (g.N % t.bn != 0) continue;
-    const long ct = cost(t.mb, t.bn);
+    const long ct = cost(t.bm, t.bn);
     if (ct < c) { c = ct; best = t; }
   }
   return best;
@@ -337,8 +299,8 @@ void enc_gemm_tc_tile(int M, int N, int K, bool fp16_out, int n_sm, int out[3]) 
   EncGemmArgs g;
   memset(&g, 0, sizeof g);
   g.M = M; g.N = N; g.K = K; g.epi = fp16_out ? ENC_EPI_BIAS_F16 : ENC_EPI_BIAS_RES_F32;
-  const TcTile t = pick_tile(g, n_sm > 0 ? n_sm : 148);
-  out[0] = t.mb * TC_BM; out[1] = t.bn; out[2] = t.stages;
+  const TcTile t = pick_tile(g, n_sm > 0 ? n_sm : 132);
+  out[0] = t.bm; out[1] = t.bn; out[2] = t.stages;
 }
 
 // `a_rows` = rows of the A view that may be touched (the allocation is padded accordingly)
@@ -362,11 +324,11 @@ cudaError_t enc_gemm_tc(const EncGemmArgs& g, int a_rows, cudaStream_t s, int64_
     int dev = 0;
     if (cudaGetDevice(&dev) != cudaSuccess ||
         cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n_sm <= 0)
-      n_sm = 148;
+      n_sm = 132;
   }
   const TcTile t = pick_tile(g, n_sm);
   CUtensorMap ma, mw;
-  if (!get(g.A, (uint64_t)a_rows, (uint64_t)g.K, (uint64_t)g.lda, (uint32_t)(t.mb * TC_BM), &ma)) return cudaErrorInvalidValue;
+  if (!get(g.A, (uint64_t)a_rows, (uint64_t)g.K, (uint64_t)g.lda, (uint32_t)t.bm, &ma)) return cudaErrorInvalidValue;
   if (!get(g.W, (uint64_t)g.N, (uint64_t)g.K, (uint64_t)g.K, (uint32_t)t.bn, &mw)) return cudaErrorInvalidValue;
   TcArgs a;
   a.M = g.M; a.N = g.N; a.K = g.K; a.epi = g.epi; a.bias = g.bias; a.out16 = g.out16; a.ldo16 = g.ldo16;
@@ -374,13 +336,13 @@ cudaError_t enc_gemm_tc(const EncGemmArgs& g, int a_rows, cudaStream_t s, int64_
   a.vt = g.vt; a.vt_col0 = g.vt_col0; a.vt_ld = g.vt_ld;
   a.ck = g.ck; a.cv = g.cv; a.kv_spad = g.kv_spad;
   if (a.ck != nullptr && (g.epi != ENC_EPI_BIAS_F16 || (g.N >> 1) % 64 != 0)) return cudaErrorInvalidValue;
-  dim3 grid(g.N / t.bn, (g.M + t.mb * TC_BM - 1) / (t.mb * TC_BM));
+  dim3 grid(g.N / t.bn, (g.M + t.bm - 1) / t.bm);
   bool launched = false;
   cudaError_t le = cudaSuccess;
-#define WM_LAUNCH(EPI, MB, BN, ST)                                                                                       \
-  if (!launched && g.epi == EPI && t.mb == MB && t.bn == BN && t.stages == ST) {                                          \
-    le = tc_launch(enc_gemm_tc_kernel<EPI, MB, BN, ST>, grid, dim3(MB == 1 ? TC_THREADS : TC_THREADS_WIDE),               \
-                   tc_smem(MB, BN, ST), s, g.pdl != 0, ma, mw, a);                                                        \
+#define WM_LAUNCH(EPI, BM, BN, ST)                                                                                       \
+  if (!launched && g.epi == EPI && t.bm == BM && t.bn == BN && t.stages == ST) {                                          \
+    le = tc_launch(enc_gemm_tc_kernel<EPI, BM, BN, ST>, grid, dim3(TC_THREADS), tc_smem(BM, BN, ST), s, g.pdl != 0, ma,  \
+                   mw, a);                                                                                               \
     launched = true;                                                                                                     \
   }
   WM_TC_ALL(WM_LAUNCH)

@@ -73,10 +73,10 @@ struct wm_handle {
   int64_t launches_a[WM_MAX_T + 1] = {0};
   int64_t launches_tail = 0, launches_b = 0;
   int decode_mode = 0;
-  int enc_gemm_impl = 0;   // 0 = mma.sync kernel, 1 = tcgen05/TMA kernel
+  int enc_gemm_impl = 0;   // 0 = mma.sync kernel, 1 = wgmma/TMA kernel
   int enc_pdl = 1;         // encoder kernels launched with programmatic stream serialization (option "enc_pdl" = 0: plain launches)
-  int enc_gemm_tile = 0;   // tcgen05 kernel: 0 = tile shape picked per GEMM, 1 = 128-row tiles only (option "enc_gemm" = 2)
-  int enc_attn_impl = 0;   // 0 = mma.sync flash attention, 1 = tcgen05/TMA/TMEM attention
+  int enc_gemm_tile = 0;   // wgmma kernel: 0 = tile shape picked per GEMM, 1 = 128 x 128 tiles only (option "enc_gemm" = 2)
+  int enc_attn_impl = 0;   // 0 = mma.sync flash attention, 1 = wgmma/TMA attention
   bool tc_ok = false, attn_tc_ok = false;
   bool encoded = false;
   // pinned staging + timing
@@ -253,7 +253,7 @@ extern "C" int wm_create(const wm_config* cfg, int device, wm_handle** out) {
   CK(cudaSetDevice(device));
   cudaDeviceProp prop;
   CK(cudaGetDeviceProperties(&prop, device));
-  if (prop.major < 10) return fail(h, WM_ERR_UNSUPPORTED, "this engine is built for sm_100a (B200) only");
+  if (prop.major != 9 || prop.minor != 0) return fail(h, WM_ERR_UNSUPPORTED, "this engine is built for sm_90a (H100) only");
   h->n_sm = prop.multiProcessorCount;
   h->n_cta = h->n_sm;
   CK(cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking));
@@ -342,7 +342,7 @@ extern "C" int wm_create(const wm_config* cfg, int device, wm_handle** out) {
   }
   CK(enc_gemm_configure());
   h->tc_ok = (enc_gemm_tc_configure() == cudaSuccess);
-  h->enc_gemm_impl = h->tc_ok ? 1 : 0;   // tcgen05/TMA GEMM by default; option "enc_gemm" = 0 selects the mma.sync kernel
+  h->enc_gemm_impl = h->tc_ok ? 1 : 0;   // wgmma/TMA GEMM by default; option "enc_gemm" = 0 selects the mma.sync kernel
   h->attn_tc_ok = (enc_attention_tc_configure() == cudaSuccess);
   h->enc_attn_impl = h->attn_tc_ok ? 1 : 0;   // likewise option "enc_attn"
   (void)cudaGetLastError();
@@ -588,7 +588,7 @@ static int run_encoder(wm_handle* h) {
     memset(&a, 0, sizeof a);
     a.A = h->ln16; a.lda = d; a.W = wptr<__half>(h, p + "qkv_w"); a.bias = wptr<float>(h, p + "qkv_b");
     a.M = S; a.N = 3 * d; a.K = d; a.epi = ENC_EPI_BIAS_F16; a.out16 = h->qkv16; a.ldo16 = 3 * d;
-    const bool vt_fused = (h->enc_attn_impl == 1 && h->enc_gemm_impl == 1);   // the tcgen05 GEMM epilogue writes V^T too
+    const bool vt_fused = (h->enc_attn_impl == 1 && h->enc_gemm_impl == 1);   // the wgmma GEMM epilogue writes V^T too
     if (vt_fused) { a.vt = h->vt16; a.vt_col0 = 2 * d; a.vt_ld = h->S_pad; }
     CK(gemm_dispatch(h, a, s, nl));
     if (h->enc_attn_impl == 1) CK(enc_attention_tc(h->qkv16, h->vt16, h->att16, S, h->S_pad, d, c.n_heads, vt_fused, s, nl, h->enc_pdl != 0));
@@ -615,7 +615,7 @@ static int run_encoder(wm_handle* h) {
     a.A = h->enc16; a.lda = d; a.W = wptr<__half>(h, p + "ckv_w"); a.bias = wptr<float>(h, p + "ckv_b");
     a.M = S; a.N = 2 * d; a.K = d; a.epi = ENC_EPI_BIAS_F16; a.out16 = h->qkv16; a.ldo16 = 2 * d;   // (scratch: [pos][k | v])
     if (h->enc_gemm_impl == 1 && d % 64 == 0) {
-      // the tcgen05 GEMM's epilogue writes the decode layout itself (pad entries stay zero from the allocation)
+      // the wgmma GEMM's epilogue writes the decode layout itself (pad entries stay zero from the allocation)
       a.ck = h->cross_k[i]; a.cv = h->cross_v[i]; a.kv_spad = h->S_pad;
       CK(gemm_dispatch(h, a, s, nl));
     } else {
@@ -970,8 +970,8 @@ extern "C" int wm_set_option(wm_handle* h, const char* key, int32_t value) {
     return WM_OK;
   }
   if (k == "enc_attn") {
-    if (value == 1 && !h->attn_tc_ok) return fail(h, WM_ERR_UNSUPPORTED, "tcgen05 attention unavailable (cuTensorMapEncodeTiled not found)");
-    if (value < 0 || value > 1) return fail(h, WM_ERR_INVALID, "enc_attn must be 0 (mma.sync) or 1 (tcgen05)");
+    if (value == 1 && !h->attn_tc_ok) return fail(h, WM_ERR_UNSUPPORTED, "wgmma attention unavailable (cuTensorMapEncodeTiled not found)");
+    if (value < 0 || value > 1) return fail(h, WM_ERR_INVALID, "enc_attn must be 0 (mma.sync) or 1 (wgmma)");
     h->enc_attn_impl = value;
     return WM_OK;
   }
@@ -981,10 +981,10 @@ extern "C" int wm_set_option(wm_handle* h, const char* key, int32_t value) {
     return WM_OK;
   }
   if (k == "enc_gemm") {
-    if (value == 1 && !h->tc_ok) return fail(h, WM_ERR_UNSUPPORTED, "tcgen05 GEMM unavailable (cuTensorMapEncodeTiled not found)");
+    if (value == 1 && !h->tc_ok) return fail(h, WM_ERR_UNSUPPORTED, "wgmma GEMM unavailable (cuTensorMapEncodeTiled not found)");
     if (value < 0 || value > 2)
-      return fail(h, WM_ERR_INVALID, "enc_gemm must be 0 (mma.sync), 1 (tcgen05) or 2 (tcgen05, 128-row tiles only)");
-    if (value >= 1 && !h->tc_ok) return fail(h, WM_ERR_UNSUPPORTED, "tcgen05 GEMM unavailable (cuTensorMapEncodeTiled not found)");
+      return fail(h, WM_ERR_INVALID, "enc_gemm must be 0 (mma.sync), 1 (wgmma) or 2 (wgmma, 128 x 128 tiles only)");
+    if (value >= 1 && !h->tc_ok) return fail(h, WM_ERR_UNSUPPORTED, "wgmma GEMM unavailable (cuTensorMapEncodeTiled not found)");
     h->enc_gemm_impl = value ? 1 : 0;
     h->enc_gemm_tile = value == 2 ? 1 : 0;
     return WM_OK;

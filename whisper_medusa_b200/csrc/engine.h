@@ -54,12 +54,12 @@ struct EncGemmArgs {
   __half* out16; int ldo16;     // fp16 outputs
   float* out32; int ldo32;      // fp32 residual stream (+=) or plain store
   const float* pos;             // [M, N] added after GELU (conv2)
-  __half* vt; int vt_col0, vt_ld;   // tcgen05 GEMM, ENC_EPI_BIAS_F16 only: columns >= vt_col0 also written transposed
-                                    // (vt[col - vt_col0][row], row stride vt_ld): V^T for the tcgen05 attention
-  __half* ck; __half* cv; int kv_spad;   // tcgen05 GEMM, ENC_EPI_BIAS_F16 only: the output [pos][k | v] (N = 2 d) goes to the
+  __half* vt; int vt_col0, vt_ld;   // wgmma GEMM, ENC_EPI_BIAS_F16 only: columns >= vt_col0 also written transposed
+                                    // (vt[col - vt_col0][row], row stride vt_ld): V^T for the wgmma attention
+  __half* ck; __half* cv; int kv_spad;   // wgmma GEMM, ENC_EPI_BIAS_F16 only: the output [pos][k | v] (N = 2 d) goes to the
                                          // decode layout cross_k / cross_v [head][kv_spad][72] instead of out16
-  int tile;                     // tcgen05 GEMM: 0 = tile shape picked per GEMM, 1 = 128-row tiles only (cross-check)
-  int pdl;                      // tcgen05 GEMM: launch with programmatic stream serialization (tc_common.cuh)
+  int tile;                     // wgmma GEMM: 0 = tile shape picked per GEMM, 1 = 128 x 128 tiles only (cross-check)
+  int pdl;                      // wgmma GEMM: launch with programmatic stream serialization (tc_common.cuh)
 };
 cudaError_t enc_gemm(const EncGemmArgs& a, cudaStream_t s, int64_t* n_launch);
 cudaError_t enc_gemm_configure();
@@ -68,17 +68,17 @@ cudaError_t enc_gemm_configure();
 cudaError_t enc_layernorm(const float* x, const float* g, const float* b, __half* y16, float* y32, int M, int d,
                           cudaStream_t s, int64_t* n_launch, bool pdl = false);
 
-// ---- enc_gemm_tc.cu (tcgen05 + TMA + TMEM) ----
+// ---- enc_gemm_tc.cu (wgmma + TMA) ----
 cudaError_t enc_gemm_tc(const EncGemmArgs& a, int a_rows, cudaStream_t s, int64_t* n_launch);
 cudaError_t enc_gemm_tc_configure();
-// tile shape {rows, columns, ring stages} the tcgen05 GEMM picks for an M x N x K product (host logic only)
+// tile shape {rows, columns, ring stages} the wgmma GEMM picks for an M x N x K product (host logic only)
 void enc_gemm_tc_tile(int M, int N, int K, bool fp16_out, int n_sm, int out[3]);
 
 // ---- enc_attn.cu ----
 // qkv: fp16 [S_pad, 3d] (q pre-scaled | k | v); out: fp16 [S_pad, d]; full (non-causal) attention over S keys
 cudaError_t enc_attention(const __half* qkv, __half* out, int S, int d, int H, cudaStream_t s, int64_t* n_launch);
 
-// ---- enc_attn_tc.cu (tcgen05 + TMA + TMEM) ----
+// ---- enc_attn_tc.cu (wgmma + TMA) ----
 // qkv as above; vt: scratch fp16 [d][S_pad] (V transposed, written here); out: fp16 [S_pad, d]
 // vt_ready: the QKV GEMM already wrote V^T (EncGemmArgs::vt); otherwise a transpose kernel runs first
 cudaError_t enc_attention_tc(const __half* qkv, __half* vt, __half* out, int S, int S_pad, int d, int H, bool vt_ready,

@@ -1,4 +1,4 @@
-// Log-mel frontend (sm_100a): framing -> hann -> 400-point real DFT -> power -> slaney mel ->
+// Log-mel frontend (sm_90a): framing -> hann -> 400-point real DFT -> power -> slaney mel ->
 // log10 -> global max floor -> (x+4)/4.  Follows HF feature_extraction_whisper.py:135-164
 // (_torch_extract_fbank_features): torch.stft(n_fft=400, hop=160, hann, center=True, reflect),
 // |.|^2, drop the last frame, mel_filters.T @ magnitudes, clamp(1e-10).log10(), max(x, max-8), (x+4)/4.

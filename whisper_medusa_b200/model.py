@@ -170,7 +170,7 @@ class WhisperMedusaModel:
         """
         device = torch.device(device)
         if device.type != "cuda":
-            raise EngineError("WhisperMedusaModel (B200 engine) runs on CUDA devices only; there is no CPU path")
+            raise EngineError("WhisperMedusaModel (H100 engine) runs on CUDA devices only; there is no CPU path")
         index = device.index if device.index is not None else torch.cuda.current_device()
         lib = _lib.load()
         if self._handle is not None:
@@ -254,7 +254,7 @@ class WhisperMedusaModel:
         _lib.load().wm_set_decode_mode(self._handle, {"graph": 0, "persistent_simple": 1, "persistent": 2}[mode])
 
     def set_option(self, key: str, value: int) -> None:
-        """Engine options (``wm_set_option``): ``enc_gemm`` 0 = mma.sync, 1 = tcgen05/TMA/TMEM encoder GEMM."""
+        """Engine options (``wm_set_option``): ``enc_gemm`` 0 = mma.sync, 1 = wgmma/TMA encoder GEMM."""
         self._require_engine()
         lib = _lib.load()
         _check(lib, self._handle, lib.wm_set_option(self._handle, key.encode(), int(value)), f"wm_set_option({key})")
@@ -417,7 +417,7 @@ class WhisperMedusaModel:
                  "decoder_input_ids"}
         unknown = sorted(set(kwargs) - known)
         if unknown:
-            raise NotImplementedError(f"generate() options not implemented by the B200 engine: {unknown}")
+            raise NotImplementedError(f"generate() options not implemented by the H100 engine: {unknown}")
 
     def generate_from_pcm(self, pcm: Union[np.ndarray, torch.Tensor], language: Optional[str] = None,
                           task: Optional[str] = None, temperature=None, **kwargs) -> torch.Tensor:

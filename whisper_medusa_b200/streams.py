@@ -2,7 +2,7 @@
 ``whisper_medusa/models/model.py:1451``, and decodes streams back to back).
 
 One speculative iteration is a chain of ~260 dependent stages, each bounded by on-chip latencies, not by HBM: a
-single stream on all 148 SMs keeps the memory system ~17 % busy.  A ``StreamGroup`` therefore partitions the SMs:
+single stream on all SMs leaves most of the memory bandwidth unused.  A ``StreamGroup`` therefore partitions the SMs:
 S engine handles share ONE copy of the packed weights (``wm_weights_device_ptr`` -> ``wm_adopt_weights``), each runs its
 persistent decode kernel on ``n_sm / S`` CTAs (option ``decode_ctas``) and on its own CUDA stream, so S cooperative
 kernels are co-resident and S weight streams are in flight at once.  Every stream computes exactly what it computes
