@@ -49,7 +49,8 @@ struct ChunkDesc {
 struct alignas(16) CtaStage {
   int stage, mode, layer;   // StageId, pass mode, decoder layer
   int epi;                  // GEMM stages: epilogue kind
-  int ln;                   // 1: the activations go through LayerNorm (its vectors arrive via nx_g/nx_b of the previous record)
+  int ln;                   // 1: the activations go through LayerNorm (gamma arrives via nx_g of the previous record; bias
+                            //    points at the {b'_n, c_n} pairs of the folded beta / gamma, dec_fold_layernorms)
   int x_ld;                 // row stride of X in floats
   int x_rows_fixed;         // 0: the pass's T rows
   int n_begin, n_rows;      // W rows of this CTA
@@ -57,13 +58,14 @@ struct alignas(16) CtaStage {
   int segs, seg, block;     // K split (FC2): segs > 1
   int pf_bias_lines;        // 128-byte lines of pf_bias
   const float* X;           // activation rows (fp32), already offset by x_row0 and the k segment
-  const float* bias;        // [N] or null
+  const float* bias;        // [N] or null (LayerNorm stages: float2 [N])
   float* out;
-  const float* nx_g;        // LayerNorm vectors of the NEXT instruction (null: it has none)
-  const float* nx_b;
+  const float* nx_g;        // LayerNorm gamma of the NEXT instruction (null: it has none)
   const float* pf_bias;     // this CTA's bias slice of the next GEMM stage (L2 prefetch)
-  int presplit;             // 1: X was written by its producer in the fp16 hi/lo operand format (no split pass)
+  int presplit;             // 1: X was written by its producer in the fp16 hi/lo operand format (no split pass;
+                            //    LayerNorm stages: X = xg, the statistics come from the fp32 rows of x)
   int out_split;            // 1: the epilogue writes `out` in that format (the consumer is a presplit stage)
+  float* out_gx;            // residual epilogues: also write nx_g o out in that format here (the next stage's xg)
   int pad_[2];
 };
 static_assert(sizeof(CtaStage) == 128, "CtaStage must be one 128-byte line");
@@ -239,6 +241,7 @@ struct alignas(16) DecModel {   // (copied to shared memory in 16-byte pieces by
   const float* pen_tab;     // [WM_MAX_POS + 32]: (factor^(L-start) - 1) as f32, 0 when inactive
   // activations (fp32)
   float* x;        // [WM_MAX_T, d] residual stream
+  float* xg;       // [WM_MAX_T, d] gamma o x in the MMA operand format, for the LayerNorm GEMM that follows (ring kernel)
   float* q;        // [WM_MAX_T, d]
   float* attn;     // [WM_MAX_T, d]
   float* ffn_h;    // [WM_MAX_T, ffn]

@@ -1517,24 +1517,74 @@ void dec_build_chunk_table(const DecModel& hm, int ncta, std::vector<ChunkDesc>&
   }
 }
 
+// Derived vectors of the LayerNorm-fed GEMMs (QKV, cross-Q, FC1) of the ring kernel, {b'_n, c_n} with
+//     c_n = sum_k gamma_k W_nk,   b'_n = b_n + sum_k beta_k W_nk
+// so that LN(x) W^T + b = rstd * ((gamma o x) W^T - mu * c) + b' (stage_gemm_ring).  Layout per decoder layer (the Medusa
+// block included): QKV [3d] | cross-Q [d] | FC1 [ffn] float2.
+size_t dec_ln_fold_len(int n_dec, int d, int ffn) { return (size_t)n_dec * (4 * (size_t)d + ffn); }
+static size_t ln_fold_offset(int stage, int layer, int d, int ffn) {
+  const size_t base = (size_t)layer * (4 * (size_t)d + ffn);
+  return base + (stage == ST_QKV ? 0 : stage == ST_CROSS_Q ? 3 * (size_t)d : 4 * (size_t)d);
+}
+
+// One warp per row of W: lane l sums k = l, l+32, ... in fp64, then a fixed butterfly; rounded once to fp32.  The order
+// does not depend on the launch, so every engine and every rank derives the same bits from the same weights.
+__global__ void __launch_bounds__(256) ln_fold_kernel(const __half* __restrict__ W, const float* __restrict__ gamma,
+                                                      const float* __restrict__ beta, const float* __restrict__ bias, int N, int K,
+                                                      float2* __restrict__ out) {
+  const int n = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  if (n >= N) return;
+  const __half* w = W + (size_t)n * K;
+  double c = 0.0, e = 0.0;
+  for (int k = lane; k < K; k += 32) {
+    const double wk = (double)__half2float(w[k]);
+    c += (double)gamma[k] * wk;
+    e += (double)beta[k] * wk;
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    c += __shfl_xor_sync(0xffffffffu, c, o);
+    e += __shfl_xor_sync(0xffffffffu, e, o);
+  }
+  if (lane == 0) out[n] = make_float2((float)((bias ? (double)bias[n] : 0.0) + e), (float)c);
+}
+
+cudaError_t dec_fold_layernorms(const DecModel& hm, int n_dec, float2* out, cudaStream_t s) {
+  const PassGeom dyn{-1, 0};
+  for (int l = 0; l < n_dec; ++l)
+    for (const int stage : {ST_QKV, ST_CROSS_Q, ST_FC1}) {
+      const GemmDesc g = make_gemm_desc(&hm, stage, MODE_B, l, &dyn);
+      ln_fold_kernel<<<(g.N + 7) / 8, 256, 0, s>>>(g.W, g.ln_g, g.ln_b, g.bias, g.N, g.K,
+                                                   out + ln_fold_offset(stage, l, hm.d, hm.ffn));
+    }
+  return cudaGetLastError();
+}
+
 // Resolved stage records of the ring kernel: tab[ip * ncta + cta] (see CtaStage in common.cuh).
-void dec_build_stage_table(const DecModel& hm, int ncta, std::vector<CtaStage>& tab) {
+void dec_build_stage_table(const DecModel& hm, const float2* ln_fold, int ncta, std::vector<CtaStage>& tab) {
   std::vector<int> flat;
   int poff[4];
   dec_build_program(hm.n_layers, hm.has_block, flat, poff);
   const int n = poff[3];
   tab.assign((size_t)n * ncta, CtaStage{});
   const PassGeom dyn{-1, 0};   // T = -1: "the rows of the pass" (resolved on the device)
+  // bias the ring kernel reads for a GEMM stage: LayerNorm stages read the {b'_n, c_n} pairs (8 bytes per row)
+  auto ring_bias = [&](const GemmDesc& g, int stage, int layer, size_t& row_bytes) -> const float* {
+    if (g.xsrc == XS_LN) {
+      row_bytes = sizeof(float2);
+      return reinterpret_cast<const float*>(ln_fold + ln_fold_offset(stage, layer, hm.d, hm.ffn));
+    }
+    row_bytes = sizeof(float);
+    return g.bias;
+  };
   for (int ip = 0; ip < n; ++ip) {
     const int stage = flat[ip * 3], mode = flat[ip * 3 + 1], layer = flat[ip * 3 + 2];
-    // LayerNorm vectors of the next instruction (bulk-copied into shared memory while this one ends) ...
-    const float* nx_g = nullptr; const float* nx_b = nullptr;
-    const bool list_end = (ip + 1 == poff[1] || ip + 1 == poff[2] || ip + 1 == poff[3]);
+    // LayerNorm gamma of the next instruction (bulk-copied into shared memory while this one runs) ...
+    const float* nx_g = nullptr;
     if (ip + 1 < n && is_gemm_stage(flat[(ip + 1) * 3])) {
       const GemmDesc gn = make_gemm_desc(&hm, flat[(ip + 1) * 3], flat[(ip + 1) * 3 + 1], flat[(ip + 1) * 3 + 2], &dyn);
-      if (gn.xsrc == XS_LN) { nx_g = gn.ln_g; nx_b = gn.ln_b; }
+      if (gn.xsrc == XS_LN) nx_g = gn.ln_g;
     }
-    (void)list_end;
     // ... and the next GEMM stage (bias prefetch)
     int jn = -1;
     for (int jp = ip + 1; jp < n && jp < ip + 4; ++jp)
@@ -1542,13 +1592,15 @@ void dec_build_stage_table(const DecModel& hm, int ncta, std::vector<CtaStage>& 
     for (int cta = 0; cta < ncta; ++cta) {
       CtaStage& c = tab[(size_t)ip * ncta + cta];
       c.stage = stage; c.mode = mode; c.layer = layer;
-      c.nx_g = nx_g; c.nx_b = nx_b;
+      c.nx_g = nx_g;
       if (jn >= 0) {
         const GemmDesc gn = make_gemm_desc(&hm, flat[jn * 3], flat[jn * 3 + 1], flat[jn * 3 + 2], &dyn);
         const GemmWork wn = gemm_work(gn.N, gn.K, hm.d, cta, ncta);
-        if (gn.bias && wn.n_rows > 0) {
-          const uintptr_t a0 = (uintptr_t)(gn.bias + wn.n_begin) & ~(uintptr_t)127;
-          const uintptr_t a1 = (uintptr_t)(gn.bias + wn.n_begin + wn.n_rows);
+        size_t rb = 0;
+        const float* nb = ring_bias(gn, flat[jn * 3], flat[jn * 3 + 2], rb);
+        if (nb && wn.n_rows > 0) {
+          const uintptr_t a0 = ((uintptr_t)nb + wn.n_begin * rb) & ~(uintptr_t)127;
+          const uintptr_t a1 = (uintptr_t)nb + (wn.n_begin + wn.n_rows) * rb;
           c.pf_bias = reinterpret_cast<const float*>(a0);
           c.pf_bias_lines = (int)std::min<uintptr_t>(32, (a1 - a0 + 127) / 128);
         }
@@ -1561,15 +1613,24 @@ void dec_build_stage_table(const DecModel& hm, int ncta, std::vector<CtaStage>& 
       c.X = g.X + (size_t)g.x_row0 * g.K + (size_t)wk.seg * hm.d;
       c.x_ld = g.K;
       c.x_rows_fixed = g.x_rows < 0 ? 0 : g.x_rows;
-      c.bias = g.bias;
+      size_t rb = 0;
+      c.bias = ring_bias(g, stage, layer, rb);
       c.out = g.out;
       c.n_begin = wk.n_begin; c.n_rows = wk.n_rows;
       c.N = g.N; c.ldo = g.ldo; c.out_row0 = g.out_row0;
       c.segs = wk.segs; c.seg = wk.seg; c.block = wk.block;
       // activations that only ever feed one GEMM stage travel in the MMA operand format: the attention stages and
-      // the GELU epilogue of FC1 write it, O-proj / cross-O / FC2 skip their split pass
-      c.presplit = (stage == ST_OPROJ || stage == ST_CROSS_O || stage == ST_FC2) ? 1 : 0;
+      // the GELU epilogue of FC1 write it, O-proj / cross-O / FC2 skip their split pass.  The residual stream feeds a
+      // LayerNorm GEMM: the residual epilogue before one also writes gamma o x in that format (xg), and that stage
+      // stages xg instead of x (layer 0 and the Medusa block, fed by other stages, split gamma o x themselves)
+      const bool resid = (stage == ST_OPROJ || stage == ST_CROSS_O || stage == ST_FC2);
+      c.presplit = resid ? 1 : 0;
       c.out_split = (stage == ST_FC1) ? 1 : 0;
+      if (resid && nx_g) c.out_gx = hm.xg;
+      if (c.ln && ip > 0) {
+        const int ps = flat[(ip - 1) * 3];
+        if (ps == ST_OPROJ || ps == ST_CROSS_O || ps == ST_FC2) { c.presplit = 1; c.X = hm.xg; }
+      }
     }
   }
 }

@@ -21,9 +21,9 @@
 //     only ~27 KB of L1 remain, so a register spill is an L2 round trip);
 //   * the stage record of this CTA (row range, pointers, epilogue; built by the host) is prefetched
 //     into shared memory while the previous stage runs;
-//   * activations arrive by bulk copy and are split in place (see below); the LayerNorm vectors of
-//     the next stage are bulk-copied during the barrier that precedes it; bias vectors are pulled
-//     into L2 one stage ahead and read while the MMAs run.  (A plain global load that is still in
+//   * activations arrive by bulk copy, written by their producers in the MMA operand format or split
+//     in place (see below); the LayerNorm gamma of the next stage is bulk-copied while the stage
+//     before it runs; bias vectors are pulled into L2 one stage ahead and read while the MMAs run.  (A plain global load that is still in
 //     flight at a bar.sync stalls the barrier: no long-latency ld may precede one.)
 //
 // Stages with K > d (FC2) are split over CTAs along K as well: CTA = (row block, k segment); the
@@ -163,8 +163,10 @@ struct RingGeom {
   static constexpr size_t SCRATCH_OFF = (size_t)WM_RING_G * SLOT_BYTES;
   static constexpr size_t SCRATCH = round128(cmax(cmax((size_t)16 * XS, cross_scratch_bytes()), self_attn_smem_bytes()));
   static constexpr size_t PARTIAL_OFF = SCRATCH_OFF + SCRATCH;
-  static constexpr size_t PARTIAL = round128(cmax((size_t)8 * 256 * sizeof(float), (size_t)2 * D * sizeof(float)));
-  static constexpr size_t MODEL_OFF = PARTIAL_OFF + PARTIAL;
+  static constexpr size_t PARTIAL = round128((size_t)NKS * 256 * sizeof(float));   // k-slice partials of one unit
+  static constexpr size_t GAMMA_OFF = PARTIAL_OFF + PARTIAL;
+  static constexpr size_t GAMMA = round128((size_t)D * sizeof(float));             // LayerNorm gamma of the running stage
+  static constexpr size_t MODEL_OFF = GAMMA_OFF + GAMMA;
   static constexpr size_t MODEL = round128(sizeof(DecModel));
   static constexpr size_t BAR_OFF = MODEL_OFF + MODEL;
   static constexpr size_t TOTAL = BAR_OFF + 128;
@@ -209,8 +211,15 @@ __device__ __noinline__ void ring_producer(unsigned char* ring, uint64_t* full, 
 // as fp32 rows of stride d*4 + 16 B and are split IN PLACE into the fp16 hi/lo operand format:
 // every 8-byte pair of floats (x[k], x[k+1]) becomes { half2 hi(k,k+1), half2 lo(k,k+1) }, so one
 // LDS.128 of the MMA loop fetches the hi AND lo A-fragment registers of two k-pairs.
-// LayerNorm stages: warp-per-row statistics out of shared memory, then thread-per-column
-// normalisation with gamma/beta read from the shared parameter buffer.
+// LayerNorm stages (QKV, cross-Q, FC1) are not normalised before the MMAs.  With mean mu, rstd and
+// gamma / beta of the row,
+//     LN(x) W^T + b = rstd * ((gamma o x) W^T - mu * c) + b',   c_n = sum_k gamma_k W_nk,  b'_n = b_n + sum_k beta_k W_nk
+// ({b', c} per output row are derived once per weight binding, dec_fold_layernorms).  The operand is
+// gamma o x, which needs no row statistics: the residual epilogue before a LayerNorm stage (O-proj,
+// cross-O, FC2) writes it in the operand format next to x (xg; element-wise, so the same for every
+// grid), and the stage stages xg like any presplit stage.  Stages fed otherwise (layer 0, the
+// Medusa block) split gamma o x in place.  mu / rstd: the epilogue warps, from the fp32 rows of x
+// in L2, while the rows are staged and the MMAs run.
 // Rows >= T keep stale bits: MMA rows are independent and rows >= T are never stored.
 // ---------------------------------------------------------------------------------------------
 __device__ __forceinline__ uint4 split_hilo4(float4 y) {
@@ -230,29 +239,23 @@ __device__ __forceinline__ float xbuf_value(const unsigned char* xb, int xs, int
   return __half2float(p[0]) + __half2float(p[2]);
 }
 
-#ifndef WM_LN_MODE
-#define WM_LN_MODE 1
-#endif
-#if WM_LN_MODE == 2
-#define WM_LN_INLINE __noinline__
-#else
-#define WM_LN_INLINE __forceinline__
-#endif
-// LayerNorm of the landed activation rows, ONE pass: warp per row, the row lives in registers (lane l holds float4
-// columns l, l+32, ...: the summation order of the two-pass statistics is unchanged), normalised with gamma / beta from
-// the shared parameter buffer and written back in the fp16 hi/lo operand format.
+// LayerNorm statistics {mu, rstd} of the fp32 rows X (row stride ld, L2-coherent loads: the staged rows are gamma o x):
+// warp w of nw takes rows w, w + nw, ...; lane l sums float4 columns l, l+32, ... of its row held in registers (two
+// passes: mean, then the centred squares).
 template <int D>
-__device__ WM_LN_INLINE void ring_layernorm_rows(unsigned char* xb, const float* partial, int T) {
+__device__ __forceinline__ void ring_row_stats(const float* X, int ld, float2* stat, int T, int w, int nw) {
   using G = RingGeom<D>;
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  constexpr int nwarps = WM_DEC_THREADS >> 5;
-  for (int r = warp; r < T; r += nwarps) {
-    uint4* row = reinterpret_cast<uint4*>(xb + (size_t)r * G::XS) + lane;
+  const int lane = threadIdx.x & 31;
+  for (int r = w; r < T; r += nw) {
+    const float* x = X + (size_t)r * ld + 4 * lane;
     float4 v[G::NV];
+#pragma unroll
+    for (int i = 0; i < G::NV; ++i)
+      if (i * 32 + lane < G::NV4) v[i] = ldcg_f4(x + i * 128);
     float s = 0.f;
 #pragma unroll
     for (int i = 0; i < G::NV; ++i)
-      if (i * 32 + lane < G::NV4) { v[i] = *reinterpret_cast<const float4*>(row + i * 32); s += (v[i].x + v[i].y) + (v[i].z + v[i].w); }
+      if (i * 32 + lane < G::NV4) s += (v[i].x + v[i].y) + (v[i].z + v[i].w);
     const float mean = warp_sum(s) / (float)D;
     float q = 0.f;
 #pragma unroll
@@ -262,27 +265,18 @@ __device__ WM_LN_INLINE void ring_layernorm_rows(unsigned char* xb, const float*
         q += (a * a + b * b) + (c * c + e * e);
       }
     const float rstd = rsqrtf(warp_sum(q) / (float)D + 1e-5f);
-#pragma unroll
-    for (int i = 0; i < G::NV; ++i)
-      if (i * 32 + lane < G::NV4) {
-        const float4 gg = reinterpret_cast<const float4*>(partial)[i * 32 + lane];
-        const float4 bb = reinterpret_cast<const float4*>(partial)[G::NV4 + i * 32 + lane];
-        float4 y;
-        y.x = (v[i].x - mean) * rstd * gg.x + bb.x;
-        y.y = (v[i].y - mean) * rstd * gg.y + bb.y;
-        y.z = (v[i].z - mean) * rstd * gg.z + bb.z;
-        y.w = (v[i].w - mean) * rstd * gg.w + bb.w;
-        row[i * 32] = split_hilo4(y);
-      }
+    if (lane == 0) stat[r] = make_float2(mean, rstd);
   }
 }
+
+__device__ __forceinline__ float4 mul4(float4 a, float4 b) { return make_float4(a.x * b.x, a.y * b.y, a.z * b.z, a.w * b.w); }
 
 // per-thread state of the compute warps that survives across stages (uniform over the CTA)
 struct RingState {
   int slot;            // ring slot of the next chunk to consume
   unsigned int par;    // its `full` parity
   unsigned int xpar;   // parity of the activation-copy barrier
-  unsigned int ppar;   // parity of the LayerNorm-vector barrier
+  unsigned int ppar;   // parity of the LayerNorm-gamma barrier
 };
 
 // ---------------------------------------------------------------------------------------------
@@ -293,19 +287,18 @@ __device__ __forceinline__ void stage_gemm_ring(RingState& rs, unsigned char* sm
                                                 int Tpass, int base, unsigned long long* pr) {
   using G = RingGeom<D>;
   __shared__ int s_last;
-#if WM_LN_MODE == 0
-  __shared__ float2 s_stat[WM_MAX_T];
-#endif
+  __shared__ float2 s_stat[WM_MAX_T];   // LayerNorm stages: {mu, rstd} of the token rows
   const int n_rows = sd->n_rows;
   unsigned char* const xb = smem + G::SCRATCH_OFF;
   float* const partial = reinterpret_cast<float*>(smem + G::PARTIAL_OFF);
+  const float* const gamma = reinterpret_cast<const float*>(smem + G::GAMMA_OFF);
   uint64_t* const full = reinterpret_cast<uint64_t*>(smem + G::BAR_OFF);
   uint64_t* const empty = full + WM_RING_G;
   uint64_t* const xbar = empty + WM_RING_G;
   uint64_t* const pbar = xbar + 1;
   if (n_rows == 0) {
-    // no rows for this CTA (narrow models; the chunk table has no entry either) -- but the LayerNorm vectors
-    // were sent to every CTA: consume that phase
+    // no rows for this CTA (narrow models; the chunk table has no entry either) -- but the LayerNorm gamma
+    // was sent to every CTA: consume that phase
     if (sd->ln) { while (!mbar_try_wait(pbar, rs.ppar)) { } rs.ppar ^= 1u; }
     return;
   }
@@ -331,68 +324,45 @@ __device__ __forceinline__ void stage_gemm_ring(RingState& rs, unsigned char* sm
     // this CTA's bias slice of the NEXT GEMM stage -> L2 (biases are cold: 2 GB of weights pass through L2 per iteration)
     if (lane < sd->pf_bias_lines) prefetch_l2(reinterpret_cast<const unsigned char*>(sd->pf_bias) + (size_t)lane * 128);
   }
+  // LayerNorm stages: the epilogue warps compute the statistics from the fp32 rows of x in L2 while the rows are staged
+  // (published behind named barrier 4, which only the epilogue warps join)
+  if (ln && warp >= G::NKS) ring_row_stats<D>(m->x, D, s_stat, T, warp - G::NKS, nwarps - G::NKS);
   while (!mbar_try_wait(xbar, rs.xpar)) { }
   rs.xpar ^= 1u;
   if (pr) pr[8] = global_timer_ns();
-#if WM_LN_MODE != 0
+  // every thread has seen the rows land; only a split pass makes the CTA wait for one another
   if (ln) {
-    // gamma / beta were bulk-copied into the (idle) partial buffer during the preceding barrier
+    // gamma was bulk-copied into its region during the preceding barrier
     while (!mbar_try_wait(pbar, rs.ppar)) { }
     rs.ppar ^= 1u;
     if (pr) pr[9] = global_timer_ns();
-    ring_layernorm_rows<D>(xb, partial, T);
-  } else
-#else
-  if (ln) {
-    // statistics: one warp per row, lane l sums float4 columns l, l+32, ... (two passes over shared memory)
-    for (int r = warp; r < T; r += nwarps) {
-      const float4* x4 = reinterpret_cast<const float4*>(xb + (size_t)r * G::XS) + lane;
-      float s = 0.f;
-#pragma unroll
-      for (int i = 0; i < G::NV; ++i)
-        if (i * 32 + lane < G::NV4) { const float4 v = x4[i * 32]; s += (v.x + v.y) + (v.z + v.w); }
-      const float mean = warp_sum(s) / (float)D;
-      float q = 0.f;
-#pragma unroll
-      for (int i = 0; i < G::NV; ++i)
-        if (i * 32 + lane < G::NV4) {
-          const float4 v = x4[i * 32];
-          const float a = v.x - mean, b = v.y - mean, c = v.z - mean, e = v.w - mean;
-          q += (a * a + b * b) + (c * c + e * e);
-        }
-      const float rstd = rsqrtf(warp_sum(q) / (float)D + 1e-5f);
-      if (lane == 0) s_stat[r] = make_float2(mean, rstd);
-    }
-    // gamma / beta were bulk-copied into the (idle) partial buffer during the preceding barrier
-    while (!mbar_try_wait(pbar, rs.ppar)) { }
-    rs.ppar ^= 1u;
-    cta_sync();
-    if (pr) pr[9] = global_timer_ns();
+  }
+  if (ln && !sd->presplit) {
+    // gamma o x -> operand format in place: thread per float4 column, the loads of 4 rows in flight together
+    static_assert(G::NV4 <= WM_DEC_THREADS, "one thread per float4 column");
     if (tid < G::NV4) {
-      const float4 gg = reinterpret_cast<const float4*>(partial)[tid];
-      const float4 bb = reinterpret_cast<const float4*>(partial)[G::NV4 + tid];
-      for (int r = 0; r < T; ++r) {
-        uint4* p = reinterpret_cast<uint4*>(xb + (size_t)r * G::XS) + tid;
-        const float4 v = *reinterpret_cast<const float4*>(p);
-        const float2 st = s_stat[r];
-        float4 y;
-        y.x = (v.x - st.x) * st.y * gg.x + bb.x;
-        y.y = (v.y - st.x) * st.y * gg.y + bb.y;
-        y.z = (v.z - st.x) * st.y * gg.z + bb.z;
-        y.w = (v.w - st.x) * st.y * gg.w + bb.w;
-        *p = split_hilo4(y);
+      const float4 g = reinterpret_cast<const float4*>(gamma)[tid];
+      for (int r0 = 0; r0 < T; r0 += 4) {
+        unsigned char* const rows = xb + (size_t)r0 * G::XS + (size_t)tid * 16;
+        float4 v[4];
+#pragma unroll
+        for (int r = 0; r < 4; ++r)
+          if (r0 + r < T) v[r] = *reinterpret_cast<const float4*>(rows + (size_t)r * G::XS);
+#pragma unroll
+        for (int r = 0; r < 4; ++r)
+          if (r0 + r < T) *reinterpret_cast<uint4*>(rows + (size_t)r * G::XS) = split_hilo4(mul4(g, v[r]));
       }
     }
-  } else
-#endif
-  if (!sd->presplit) {
+    if (pr) pr[10] = global_timer_ns();
+    cta_sync();
+  } else if (!ln && !sd->presplit) {
     // flat over the buffer (the 16-byte row pad is converted along: no index arithmetic)
     uint4* p = reinterpret_cast<uint4*>(xb);
     const int n16 = T * (G::XS >> 4);
     for (int idx = tid; idx < n16; idx += WM_DEC_THREADS) p[idx] = split_hilo4(*reinterpret_cast<const float4*>(p + idx));
+    if (pr) pr[10] = global_timer_ns();
+    cta_sync();
   }
-  if (pr) pr[10] = global_timer_ns();
-  cta_sync();
   if (pr) pr[3] = global_timer_ns();
   const int units = (n_rows + 15) >> 4;
   const bool ksplit = sd->segs > 1;
@@ -454,22 +424,33 @@ __device__ __forceinline__ void stage_gemm_ring(RingState& rs, unsigned char* sm
     const int etid = tid - G::NKS * 32;
     constexpr int NOUT = (256 + NE - 1) / NE;   // outputs per epilogue thread and unit
     // this thread's bias / residual values of a unit are requested before its partials are awaited: the loads are in
-    // flight while the MMA warps work
-    float bias_v[NOUT], old[NOUT];
-    auto fetch = [&](int u, float* bv, float* ov) {
+    // flight while the MMA warps work.  aux = the residual (EPI_RESID) or, in LayerNorm stages, c_n (sd->bias then
+    // points at the {b'_n, c_n} pairs)
+    float bias_v[NOUT], aux[NOUT];
+    auto fetch = [&](int u, float* bv, float* av) {
       const int nvalid = min(16, n_rows - u * 16);
 #pragma unroll
       for (int k = 0; k < NOUT; ++k) {
         const int o = etid + k * NE, token = o >> 4, rloc = o & 15;
-        bv[k] = 0.f; ov[k] = 0.f;
+        bv[k] = 0.f; av[k] = 0.f;
         if (o < 256 && token < T && rloc < nvalid && !ksplit) {
           const float* bias = sd->bias;
-          if (bias) bv[k] = bias[n_begin + u * 16 + rloc];
-          if (epi == EPI_RESID) ov[k] = ldcg_f(&sd->out[(size_t)token * sd->ldo + n_begin + u * 16 + rloc]);
+          const int row = n_begin + u * 16 + rloc;
+          if (ln) {
+            const float2 bc = reinterpret_cast<const float2*>(bias)[row];
+            bv[k] = bc.x; av[k] = bc.y;
+          } else {
+            if (bias) bv[k] = bias[row];
+            if (epi == EPI_RESID) av[k] = ldcg_f(&sd->out[(size_t)token * sd->ldo + row]);
+          }
         }
       }
     };
-    fetch(0, bias_v, old);
+    fetch(0, bias_v, aux);
+    // residual epilogues before a LayerNorm stage: that stage's gamma is on its way into the gamma region (the copy is
+    // issued when this stage begins; its phase is consumed by the LayerNorm stage)
+    if (sd->out_gx) while (!mbar_try_wait(pbar, rs.ppar)) { }
+    if (ln) asm volatile("bar.sync 4, %0;" ::"n"(NE) : "memory");   // LayerNorm statistics written
     for (int u = 0; u < units; ++u) {
       const int nvalid = min(16, n_rows - u * 16);
       asm volatile("bar.sync 2, %0;" ::"n"(WM_DEC_THREADS) : "memory");   // partials of unit u are written
@@ -494,19 +475,28 @@ __device__ __forceinline__ void stage_gemm_ring(RingState& rs, unsigned char* sm
         if (!(o < 256 && token < T && rloc < nvalid)) continue;
         const int row = n_begin + u * 16 + rloc;
         const float s = sum[k];
+        float y;   // the GEMM output with its bias
+        if (ln) {
+          const float2 st = s_stat[token];
+          y = st.y * (s - st.x * aux[k]) + bias_v[k];
+        } else {
+          y = s + bias_v[k];
+        }
         // common epilogues inline; the Medusa-head ones are rare
         if (ksplit) {
           m->gemm_part[((size_t)sd->seg * 16 + token) * sd->N + row] = s;
         } else if (epi == EPI_RESID) {
-          out[(size_t)token * ldo + row] = old[k] + (s + bias_v[k]);
+          const float v = aux[k] + y;
+          out[(size_t)token * ldo + row] = v;
+          if (sd->out_gx) store_split(sd->out_gx + (size_t)token * ldo, row, gamma[row] * v);
         } else if (epi == EPI_STORE || epi == EPI_LOGITS) {
-          out[(size_t)token * ldo + row] = s + bias_v[k];
+          out[(size_t)token * ldo + row] = y;
         } else if (epi == EPI_GELU) {
-          const float v = gelu_erf(s + bias_v[k]);
+          const float v = gelu_erf(y);
           if (sd->out_split) store_split(out + (size_t)token * ldo, row, v);
           else out[(size_t)token * ldo + row] = v;
         } else if (epi == EPI_QKV) {
-          const float v = s + bias_v[k];
+          const float v = y;
           const DecLayer& L = m->layers[sd->layer];
           if (row < D) out[(size_t)token * ldo + row] = v;
           else if (row < 2 * D) L.self_k[(size_t)(base + token) * D + (row - D)] = __float2half_rn(v);
@@ -514,12 +504,12 @@ __device__ __forceinline__ void stage_gemm_ring(RingState& rs, unsigned char* sm
         } else if (epi == EPI_HEADS_A) {
           // head `row / d` on the newest token's hidden state: x + SiLU(W x + b)  (medusa ResBlock)
           const int head = row / D, n = row - head * D;
-          out[(size_t)(sd->out_row0 + head) * ldo + n] = xbuf_value(xb, G::XS, 0, n) + silu(s + bias_v[k]);
+          out[(size_t)(sd->out_row0 + head) * ldo + n] = xbuf_value(xb, G::XS, 0, n) + silu(y);
         } else {   // EPI_HEAD_B
-          out[(size_t)token * ldo + row] = xbuf_value(xb, G::XS, token, row) + silu(s + bias_v[k]);
+          out[(size_t)token * ldo + row] = xbuf_value(xb, G::XS, token, row) + silu(y);
         }
       }
-      if (u + 1 < units) fetch(u + 1, bias_v, old);   // (fetching TWO units ahead into a second register set timed slower)
+      if (u + 1 < units) fetch(u + 1, bias_v, aux);   // (fetching TWO units ahead into a second register set timed slower)
     }
     for (int u = 0; u < units; ++u)
       if (++rs.slot == WM_RING_G) { rs.slot = 0; rs.par ^= 1u; }   // keep the (uniform) ring state in step with the MMA warps
@@ -536,6 +526,7 @@ __device__ __forceinline__ void stage_gemm_ring(RingState& rs, unsigned char* sm
     }
     cta_sync();
     if (s_last) {
+      if (sd->out_gx) while (!mbar_try_wait(pbar, rs.ppar)) { }   // (see the epilogue above)
       const float* bias = sd->bias;
       float* out = sd->out;
       const int ldo = sd->ldo;
@@ -557,7 +548,9 @@ __device__ __forceinline__ void stage_gemm_ring(RingState& rs, unsigned char* sm
             for (int i = 0; i < 4; ++i)
               if (s0 + i < segs) s += pv[i];
           }
-          *o = xo + (s + bv);
+          const float v = xo + (s + bv);
+          *o = v;
+          if (sd->out_gx) store_split(sd->out_gx + (size_t)t * ldo, row, gamma[row] * v);
         }
       }
     }
@@ -676,6 +669,13 @@ dec_iteration_ring_kernel(const DecModel* __restrict__ gm) {
     if (mode == MODE_A) { pgv.T = L0 - kv0; pgv.base = kv0; }
     else if (mode == MODE_B) { pgv.T = m->n_tree; pgv.base = L0; }
     else { pgv.T = 1; pgv.base = L0 - 1; }
+    // LayerNorm gamma of the next stage -> its region (last read by an earlier LayerNorm stage; a LayerNorm stage never
+    // precedes another), in flight while this stage runs: its residual epilogue (if any) reads it too
+    if (threadIdx.x == 0 && sd->nx_g != nullptr) {
+      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+      mbar_expect_tx(pbar, (uint32_t)(D * 4));
+      bulk_g2s(smem + G::GAMMA_OFF, sd->nx_g, (uint32_t)(D * 4), pbar);
+    }
     if (is_gemm_stage(stage)) {
       stage_gemm_ring<D>(rs, smem, m, sd, pgv.T, pgv.base, pr);
     } else if (stage == ST_CROSS_ATTN) {
@@ -687,15 +687,6 @@ dec_iteration_ring_kernel(const DecModel* __restrict__ gm) {
     }
     if (prof) pr[15] = global_timer_ns();
     if (fetch) reinterpret_cast<uint32_t*>(&s_desc[(ip + 1) & 1])[lane] = nxt_w;
-    // LayerNorm vectors of the next stage -> the partial buffer (idle until that stage's first MMA), in
-    // flight across the grid barrier
-    if (threadIdx.x == 0 && sd->nx_g != nullptr) {
-      float* const partial = reinterpret_cast<float*>(smem + G::PARTIAL_OFF);
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-      mbar_expect_tx(pbar, (uint32_t)(2 * D * 4));
-      bulk_g2s(partial, sd->nx_g, (uint32_t)(D * 4), pbar);
-      bulk_g2s(partial + D, sd->nx_b, (uint32_t)(D * 4), pbar);
-    }
     if (prof) pr[1] = global_timer_ns();
     epoch = grid_barrier_step<false>(m->bar, epoch, ncta);
     if (prof) pr[2] = global_timer_ns();

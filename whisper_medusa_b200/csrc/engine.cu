@@ -66,6 +66,7 @@ struct wm_handle {
   ChunkDesc* chunk_tab = nullptr;
   int* chunk_off = nullptr;
   CtaStage* stage_tab = nullptr;
+  float2* ln_fold = nullptr;     // {b'_n, c_n} of the LayerNorm-fed GEMMs of the ring kernel (derived from the weights)
   DecTree* tree = nullptr;       // device copy of the candidate tree (branching medusa_choices)
   DecHostInfo hi;
   std::map<int, cudaGraphExec_t> graph_a;  // sweep A, keyed by T
@@ -297,6 +298,7 @@ extern "C" int wm_create(const wm_config* cfg, int device, wm_handle** out) {
   CK(dalloc(&h->tree, 1));
   CK(dalloc(&m.topk_part, (size_t)WM_MAX_T * 32 * WM_TREE_MAX_TOPK * 2));
   CK(dalloc(&m.x, (size_t)WM_MAX_T * d));
+  CK(dalloc(&m.xg, (size_t)WM_MAX_T * d));
   CK(dalloc(&m.q, (size_t)WM_MAX_T * d));
   CK(dalloc(&m.attn, (size_t)WM_MAX_T * d));
   CK(dalloc(&m.ffn_h, (size_t)WM_MAX_T * f));
@@ -365,8 +367,8 @@ extern "C" int wm_destroy(wm_handle* h) {
   for (auto p : h->cross_v) F(p);
   for (auto p : h->self_k) F(p);
   for (auto p : h->self_v) F(p);
-  F(h->hm.x); F(h->hm.q); F(h->hm.attn); F(h->hm.ffn_h); F(h->hm.hidden); F(h->hm.head_h); F(h->hm.carry); F(h->hm.cross_part); F(h->hm.cross_cnt); F(h->hm.sel_part); F(h->hm.gemm_part); F(h->hm.gemm_cnt);
-  F(h->hm.topk_part); F(h->tree); F(h->hm.logits_a); F(h->hm.logits_b); F(h->st); F(h->tok_mask); F(h->pen_tab); F(h->bar); F(h->prog); F(h->prof); F(h->chunk_tab); F(h->chunk_off); F(h->stage_tab); F(h->dm);
+  F(h->hm.x); F(h->hm.xg); F(h->hm.q); F(h->hm.attn); F(h->hm.ffn_h); F(h->hm.hidden); F(h->hm.head_h); F(h->hm.carry); F(h->hm.cross_part); F(h->hm.cross_cnt); F(h->hm.sel_part); F(h->hm.gemm_part); F(h->hm.gemm_cnt);
+  F(h->hm.topk_part); F(h->tree); F(h->hm.logits_a); F(h->hm.logits_b); F(h->st); F(h->tok_mask); F(h->pen_tab); F(h->bar); F(h->prog); F(h->prof); F(h->chunk_tab); F(h->chunk_off); F(h->stage_tab); F(h->ln_fold); F(h->dm);
   if (h->wowned) F(h->wdev);
   if (h->h_state) cudaFreeHost(h->h_state);
   if (h->h_stage) cudaFreeHost(h->h_stage);
@@ -431,6 +433,11 @@ static int bind_weights(wm_handle* h) {
   m.pos = wptr<float>(h, "dec.pos");
   m.lnf_g = wptr<float>(h, "dec.lnf_g"); m.lnf_b = wptr<float>(h, "dec.lnf_b");
   m.heads_w = wptr<__half>(h, "heads_w"); m.heads_b = wptr<float>(h, "heads_b");
+  // LayerNorm beta / gamma folded through the weights they feed (ring kernel; a function of the weight values, so
+  // derived again at every binding: upload, broadcast, adoption of another engine's weights)
+  if (!h->ln_fold) CK(dalloc(&h->ln_fold, dec_ln_fold_len(h->n_dec, h->cfg.d_model, h->cfg.ffn_dim)));
+  CK(dec_fold_layernorms(m, h->n_dec, h->ln_fold, h->stream));
+  CK(cudaStreamSynchronize(h->stream));
   {
     // weight-chunk schedule of the ring producer (depends on the weight addresses)
     std::vector<ChunkDesc> tab;
@@ -445,7 +452,7 @@ static int bind_weights(wm_handle* h) {
     m.chunk_tab = h->chunk_tab;
     m.chunk_off = h->chunk_off;
     std::vector<CtaStage> stab;
-    dec_build_stage_table(m, h->n_cta, stab);
+    dec_build_stage_table(m, h->ln_fold, h->n_cta, stab);
     if (h->stage_tab) { cudaFree(h->stage_tab); h->stage_tab = nullptr; }
     CK(cudaMalloc((void**)&h->stage_tab, stab.size() * sizeof(CtaStage)));
     CK(cudaMemcpy(h->stage_tab, stab.data(), stab.size() * sizeof(CtaStage), cudaMemcpyHostToDevice));

@@ -28,8 +28,12 @@ struct ChunkDesc;
 void dec_build_chunk_table(const DecModel& hm, int ncta, std::vector<ChunkDesc>& tab, std::vector<int>& off);
 cudaError_t dec_relayout_cross_kv(const __half* kv, __half* ck, __half* cv, int S, int S_pad, int d, int H, cudaStream_t s,
                                   int64_t* n_launch);
+// {b'_n, c_n} of the LayerNorm-fed GEMMs of the ring kernel: float2 count for n_dec decoder layers, and the derivation
+// from the bound weights (enqueued on s)
+size_t dec_ln_fold_len(int n_dec, int d, int ffn);
+cudaError_t dec_fold_layernorms(const DecModel& hm, int n_dec, float2* out, cudaStream_t s);
 struct CtaStage;
-void dec_build_stage_table(const DecModel& hm, int ncta, std::vector<CtaStage>& tab);
+void dec_build_stage_table(const DecModel& hm, const float2* ln_fold, int ncta, std::vector<CtaStage>& tab);
 cudaError_t dec_launch_iteration_ring(const DecModel* dm, const DecHostInfo& hi, bool profile, cudaStream_t s);
 // phase: 0 = sweep A over T uncached rows, 1 = tail (candidates), 2 = verify sweep + accept
 cudaError_t dec_enqueue_phase(const DecModel* dm, const DecHostInfo& hi, int phase, int T, cudaStream_t s, int64_t* n_launch);
