@@ -23,6 +23,11 @@ of the reference model: for that part parity is "unpinned" (see DESIGN.md).
     reproduced (fp16 operands of the encoder GEMMs and of encoder attention, fp16 self- and
     cross-attention K/V caches).  Token-id parity is asserted against this regime; logits
     closeness is asserted against both.
+
+The decoder side (``decoder_forward``, ``medusa_logits`` and the loop in ``medusa_ref.py``) also
+runs in fp64 (``RefWeights(sd, dtype=torch.float64)``): the engine regime then still rounds the
+K/V caches to fp16 and widens them back, and everything else is fp64.  The fp32 results are
+unchanged by a bit.
 """
 from __future__ import annotations
 
@@ -42,8 +47,8 @@ LN_EPS = 1e-5
 
 
 def _r16(x: torch.Tensor) -> torch.Tensor:
-    """Round to fp16 and back (an engine rounding point)."""
-    return x.to(torch.float16).to(torch.float32)
+    """Round to fp16 and back to the working dtype (an engine rounding point)."""
+    return x.to(torch.float16).to(x.dtype)
 
 
 # --------------------------------------------------------------------------------------
@@ -123,10 +128,16 @@ def log_mel_spectrogram(pcm: np.ndarray) -> np.ndarray:
 # weights
 # --------------------------------------------------------------------------------------
 class RefWeights:
-    """fp32 view of an fp16 checkpoint state dict (reference key layout, SURVEY.md 3.1)."""
+    """View of an fp16 checkpoint state dict (reference key layout, SURVEY.md 3.1) in the working dtype.
 
-    def __init__(self, state_dict: Dict[str, torch.Tensor]):
-        self.sd = {k: v.detach().to(torch.float32) for k, v in state_dict.items()}
+    ``dtype`` is the dtype every decoder-side function computes in: fp32 (default, the reference's numerics) or
+    fp64 (an independent high-precision reference for the engine's decode path; the engine regime still rounds the
+    K/V caches to fp16 and widens them back).  The encoder is fp32-only."""
+
+    def __init__(self, state_dict: Dict[str, torch.Tensor], dtype: torch.dtype = torch.float32):
+        self.dtype = dtype
+        self.sd = {k: v.detach().to(dtype) for k, v in state_dict.items()}
+        self.ln_probe = None     # optional callable(prefix, x): sees every LayerNorm input (statistics in tests)
 
     def __getitem__(self, k: str) -> torch.Tensor:
         return self.sd[k]
@@ -138,6 +149,8 @@ class RefWeights:
         return F.linear(x, self.sd[prefix + ".weight"], self.sd.get(prefix + ".bias"))
 
     def ln(self, x: torch.Tensor, prefix: str) -> torch.Tensor:
+        if self.ln_probe is not None:
+            self.ln_probe(prefix, x)
         return F.layer_norm(x, (x.shape[-1],), self.sd[prefix + ".weight"], self.sd[prefix + ".bias"], LN_EPS)
 
 
@@ -285,7 +298,7 @@ def _decoder_layer(w: RefWeights, cfg, lp: str, li: int, x: torch.Tensor, enc: t
     h = w.ln(x, f"{lp}.encoder_attn_layer_norm")
     q = w.lin(h, f"{lp}.encoder_attn.q_proj") * (dh ** -0.5)
     if cache.cross_k[li] is None:
-        e = rq(enc)
+        e = rq(enc.to(w.dtype))
         cache.cross_k[li] = rq(w.lin(e, f"{lp}.encoder_attn.k_proj"))
         cache.cross_v[li] = rq(w.lin(e, f"{lp}.encoder_attn.v_proj"))
     scores = _split_heads(q, H) @ _split_heads(cache.cross_k[li], H).transpose(1, 2)

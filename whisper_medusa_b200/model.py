@@ -249,9 +249,13 @@ class WhisperMedusaModel:
     def set_decode_mode(self, mode: str) -> None:
         """``"graph"``: CUDA graphs of stage kernels (debug / per-stage profiling); ``"persistent"``: one
         cooperative kernel per speculative iteration with the weight ring (product path);
-        ``"persistent_simple"``: the same without the ring (grid barriers only)."""
+        ``"persistent_simple"``: the same without the ring (grid barriers only).  A mode the engine cannot run here
+        (``"persistent"`` at a decoder width without a ring-kernel instantiation) raises ``EngineError``."""
         self._require_engine()
-        _lib.load().wm_set_decode_mode(self._handle, {"graph": 0, "persistent_simple": 1, "persistent": 2}[mode])
+        lib = _lib.load()
+        rc = lib.wm_set_decode_mode(self._handle, {"graph": 0, "persistent_simple": 1, "persistent": 2}[mode])
+        if rc < 0:
+            _check(lib, self._handle, rc, f"set_decode_mode({mode!r})")
 
     def set_option(self, key: str, value: int) -> None:
         """Engine options (``wm_set_option``): ``enc_gemm`` 0 = mma.sync, 1 = wgmma/TMA encoder GEMM."""
