@@ -9,7 +9,7 @@
 #define WM_MAX_DEC_LAYERS 40
 #define WM_MAX_POS 512       // self-KV rows allocated per layer (448 + tree slack)
 #define WM_CROSS_CHUNKS 8    // cross-attention key chunks per head (flash-decoding split)
-#define WM_CH_MAX_KEYS 216   // keys per chunk (one ring slot; S = 1500 => at least 7 chunks per head)
+#define WM_CH_MAX_KEYS 256   // keys per chunk (one ring slot; S = 1500 => at least 6 chunks per head: large-v2's 20 x 6 items are one wave on 132 SMs)
 #ifndef WM_DEC_THREADS
 #define WM_DEC_THREADS 352   // compute threads per decode CTA (11 warps; the ring kernel adds a producer warp -> 384 => 168 registers)
 #endif

@@ -459,9 +459,11 @@ __device__ __forceinline__ void stage_self_attn(const DecModel* m, int mode, int
 // item = (head, chunk); all T query rows at once.  K/V rows: cross_kv[pos][0:d | d:2d] fp16.
 // The chunk that arrives last for a head folds the partials (chunk order => deterministic).
 // -----------------------------------------------------------------------------------------
-#define WM_CH_MAX WM_CH_MAX_KEYS   // keys per chunk (S = 1500 over >= 7 chunks)
-#define WM_CH_PAD 224   // rounded up to the MMA k-step (16 keys)
+#define WM_CH_MAX WM_CH_MAX_KEYS   // keys per chunk (S = 1500 over >= 6 chunks)
+#define WM_CH_PAD 256   // rounded up to the MMA k-step (16 keys)
 #define WM_SS_STRIDE (WM_CH_PAD + 8)   // score row stride in floats: 32 B (mod 128) => conflict-free 8-byte fragment loads
+static_assert(WM_CH_PAD % 16 == 0 && WM_CH_PAD >= WM_CH_MAX, "a padded key chunk must hold WM_CH_MAX keys");
+static_assert(WM_SS_STRIDE * 4 % 128 == 32, "score row stride must stay 32 B (mod 128)");
 __host__ __device__ constexpr size_t cross_attn_smem_bytes() {
   return (size_t)2 * WM_CH_PAD * 72 * sizeof(__half) + (size_t)WM_MAX_T * WM_SS_STRIDE * sizeof(float) +
          (size_t)2 * 16 * 72 * sizeof(__half) + (size_t)2 * WM_MAX_T * sizeof(float);   // K, V chunk + cross_scratch_bytes()
