@@ -107,6 +107,26 @@ int wm_encode_mel(wm_handle* h, const float* mel);
  * reference's caller does `input_features.to(device)` first, README.md:129-133).  `producer_stream` is the
  * cudaStream_t (NULL = legacy default stream) the features were produced on: the copy is ordered after it. */
 int wm_encode_mel_device(wm_handle* h, const float* mel_dev, void* producer_stream);
+/* Device twin of wm_encode_pcm: n_samples (0..480000) f32 samples @16 kHz in DEVICE memory of the handle's GPU, e.g. one
+ * window in the middle of a long recording.  Samples past the window are zero, as for host PCM, and the log-mel and
+ * encoder output are bit-identical to wm_encode_pcm on the same samples.  Ordered after `producer_stream` (as for
+ * wm_encode_mel_device). */
+int wm_encode_pcm_device(wm_handle* h, const float* pcm_dev, int32_t n_samples, void* producer_stream);
+
+/* ---- resampler (torchaudio.functional.resample with its defaults: sinc_interp_hann, lowpass_filter_width 6,
+ *      rolloff 0.99; integer rates) ------------------------------------------------------------------------------ */
+/* Mono f32 samples in DEVICE memory, n_in of them at orig_hz -> *n_out = ceil(n_in * new / orig) samples at new_hz in
+ * out_dev (orig / new: the rates divided by their gcd; out_cap >= *n_out).  Enqueued on `stream` (cudaStream_t, NULL =
+ * legacy default stream); orig_hz == new_hz is a device copy.  The handle keeps the tap table of every rate pair it
+ * has resampled; its weights need not be loaded. */
+int wm_resample(wm_handle* h, const float* in_dev, int64_t n_in, int32_t orig_hz, int32_t new_hz, float* out_dev,
+                int64_t out_cap, int64_t* n_out, void* stream);
+/* Host logic, no GPU needed: the polyphase table the resampler runs for orig_hz -> new_hz, built in fp64 and rounded
+ * once to fp32.  info4 = {orig, new, width, max_taps} after the gcd reduction.  With taps / lo / n_taps given
+ * (cap >= new * max_taps floats): phase p has n_taps[p] taps taps[p * max_taps + j] on columns lo[p] + j of
+ * torchaudio's dense [new][2 * width + orig] kernel, whose other columns are zero. */
+int wm_resample_taps(int32_t orig_hz, int32_t new_hz, float* taps, int32_t* lo, int32_t* n_taps, int64_t cap,
+                     int32_t* info4);
 
 /* ---- the speculative decode loop (model.py:404-835 + medusa_utils.py:424-671) ---------- */
 /* prompt: decoder_input_ids, 1 <= n_prompt < max_length - K - 2 (beyond 16 tokens the leading ones are cached by prefill

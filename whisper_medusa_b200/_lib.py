@@ -49,6 +49,11 @@ SYMBOLS = {
     "wm_encode_pcm": (C.c_int, [C.c_void_p, _P(C.c_float), C.c_int32]),
     "wm_encode_mel": (C.c_int, [C.c_void_p, _P(C.c_float)]),
     "wm_encode_mel_device": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),
+    "wm_encode_pcm_device": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p]),
+    "wm_resample": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_int32, C.c_void_p, C.c_int64,
+                              _P(C.c_int64), C.c_void_p]),
+    "wm_resample_taps": (C.c_int, [C.c_int32, C.c_int32, _P(C.c_float), _P(C.c_int32), _P(C.c_int32), C.c_int64,
+                                   _P(C.c_int32)]),
     "wm_generate": (C.c_int, [C.c_void_p, _P(C.c_int32), C.c_int32, _P(WmGenParams), _P(C.c_int32),
                               _P(C.c_int32), _P(C.c_int32), _P(C.c_int32)]),
     "wm_forward": (C.c_int, [C.c_void_p, _P(C.c_int32), C.c_int32, _P(C.c_float)]),

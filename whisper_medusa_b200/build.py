@@ -19,7 +19,8 @@ OBJ_DIR = os.path.join(OUT_DIR, "obj")
 LIB_PATH = os.path.join(OUT_DIR, "libwm_b200.so")
 ROOT = os.path.dirname(HERE)
 
-SOURCES = ["engine.cu", "decode.cu", "mel.cu", "enc_gemm.cu", "enc_attn.cu", "enc_gemm_tc.cu", "enc_attn_tc.cu"]
+SOURCES = ["engine.cu", "decode.cu", "mel.cu", "enc_gemm.cu", "enc_attn.cu", "enc_gemm_tc.cu", "enc_attn_tc.cu",
+           "resample.cu"]
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",

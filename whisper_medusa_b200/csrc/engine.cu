@@ -4,6 +4,7 @@
 // mel / encoder / cross-KV kernels for a clip, and drive the speculative loop (CUDA graphs of
 // stage kernels, or the persistent per-iteration kernel).  No arithmetic of the path runs on
 // the host; there is no CPU fallback.
+#include <algorithm>
 #include <cmath>
 #include <cstdio>
 #include <cstring>
@@ -90,6 +91,15 @@ struct wm_handle {
   int64_t launches[3] = {0, 0, 0};
   float last_pen_factor = 0.f;
   int last_pen_start = -2, last_pen_prompt = -1;
+  // resampler tap tables on the device, one per (orig_hz, new_hz) pair used on this handle
+  struct Resampler {
+    ResampleTable t;
+    float* taps = nullptr;   // [max_taps][nw]
+    int2* sup = nullptr;     // [nw] {lo - width, n}
+    int T = 0;
+    size_t smem = 0;
+  };
+  std::map<std::pair<int, int>, Resampler> resamplers;
 };
 
 static_assert(offsetof(DecState, tree_attn) == 60, "the 16 header words of DecState (L .. tree_attn) are patched as one 64-byte copy");
@@ -370,6 +380,7 @@ extern "C" int wm_destroy(wm_handle* h) {
   F(h->hm.x); F(h->hm.xg); F(h->hm.q); F(h->hm.attn); F(h->hm.ffn_h); F(h->hm.hidden); F(h->hm.head_h); F(h->hm.carry); F(h->hm.cross_part); F(h->hm.cross_cnt); F(h->hm.sel_part); F(h->hm.gemm_part); F(h->hm.gemm_cnt);
   F(h->hm.topk_part); F(h->tree); F(h->hm.logits_a); F(h->hm.logits_b); F(h->st); F(h->tok_mask); F(h->pen_tab); F(h->bar); F(h->prog); F(h->prof); F(h->chunk_tab); F(h->chunk_off); F(h->stage_tab); F(h->ln_fold); F(h->dm);
   if (h->wowned) F(h->wdev);
+  for (auto& kv : h->resamplers) { F(kv.second.taps); F(kv.second.sup); }
   if (h->h_state) cudaFreeHost(h->h_state);
   if (h->h_stage) cudaFreeHost(h->h_stage);
   if (h->h_init) cudaFreeHost(h->h_init);
@@ -659,6 +670,79 @@ extern "C" int wm_encode_pcm(wm_handle* h, const float* pcm, int32_t n) {
   int r = run_encoder(h);
   if (r != WM_OK) return r;
   return finish_encode(h);
+}
+
+// Device twin of wm_encode_pcm: the window is copied into the handle's PCM buffer and the rest of the buffer is zeroed,
+// so the mel kernels see exactly the samples wm_encode_pcm stages from the host.
+extern "C" int wm_encode_pcm_device(wm_handle* h, const float* pcm_dev, int32_t n, void* producer_stream) {
+  if (!h || n < 0 || n > kSamples || (!pcm_dev && n > 0)) return WM_ERR_INVALID;
+  if (!h->wready) return fail(h, WM_ERR_STATE, "weights not loaded");
+  CK(cudaSetDevice(h->device));
+  h->launches[0] = h->launches[1] = 0;
+  CK(cudaEventRecord(h->ev[5], reinterpret_cast<cudaStream_t>(producer_stream)));
+  CK(cudaStreamWaitEvent(h->stream, h->ev[5], 0));
+  CK(cudaEventRecord(h->ev[0], h->stream));
+  if (n > 0) CK(cudaMemcpyAsync(h->pcm, pcm_dev, (size_t)n * sizeof(float), cudaMemcpyDeviceToDevice, h->stream));
+  if (n < kSamples) CK(cudaMemsetAsync(h->pcm + n, 0, (size_t)(kSamples - n) * sizeof(float), h->stream));
+  CK(mel_forward(h->pcm, h->melfb, h->mel32, h->x_tm, h->gmax, h->stream, &h->launches[0]));
+  CK(cudaEventRecord(h->ev[1], h->stream));
+  int r = run_encoder(h);
+  if (r != WM_OK) return r;
+  return finish_encode(h);
+}
+
+extern "C" int wm_resample(wm_handle* h, const float* in_dev, int64_t n_in, int32_t orig_hz, int32_t new_hz,
+                           float* out_dev, int64_t out_cap, int64_t* n_out, void* stream) {
+  if (!h || !n_out || n_in < 0 || (n_in > 0 && (!in_dev || !out_dev)) || orig_hz <= 0 || new_hz <= 0 || n_in >= (int64_t(1) << 40))
+    return WM_ERR_INVALID;
+  if (h->device < 0) return fail(h, WM_ERR_STATE, "layout-only handle has no device");
+  CK(cudaSetDevice(h->device));
+  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+  if (orig_hz == new_hz) {
+    *n_out = n_in;
+    if (out_cap < n_in) return fail(h, WM_ERR_INVALID, "out_cap is smaller than the resampled length");
+    if (n_in > 0) CK(cudaMemcpyAsync(out_dev, in_dev, (size_t)n_in * sizeof(float), cudaMemcpyDeviceToDevice, s));
+    return WM_OK;
+  }
+  auto key = std::make_pair((int)orig_hz, (int)new_hz);
+  auto it = h->resamplers.find(key);
+  if (it == h->resamplers.end()) {
+    wm_handle::Resampler r;
+    if (!resample_build_table(orig_hz, new_hz, r.t))
+      return fail(h, WM_ERR_UNSUPPORTED, "rates too large after dividing by their gcd");
+    r.T = resample_block_outputs(r.t, &r.smem);
+    if (r.T == 0) return fail(h, WM_ERR_UNSUPPORTED, "downsampling ratio too large for the staged input tile");
+    const ResampleTable& t = r.t;
+    std::vector<float> tt((size_t)t.max_taps * t.nw);
+    for (int p = 0; p < t.nw; ++p)
+      for (int j = 0; j < t.max_taps; ++j) tt[(size_t)j * t.nw + p] = t.taps[(size_t)p * t.max_taps + j];
+    std::vector<int2> sup((size_t)t.nw);
+    for (int p = 0; p < t.nw; ++p) sup[p] = make_int2(t.lo[p] - t.width, t.n[p]);
+    CK(dalloc(&r.taps, tt.size()));
+    CK(dalloc(&r.sup, sup.size()));
+    CK(cudaMemcpy(r.taps, tt.data(), tt.size() * sizeof(float), cudaMemcpyHostToDevice));
+    CK(cudaMemcpy(r.sup, sup.data(), sup.size() * sizeof(int2), cudaMemcpyHostToDevice));
+    it = h->resamplers.emplace(key, r).first;
+  }
+  const wm_handle::Resampler& r = it->second;
+  const int64_t m = resample_out_len(n_in, r.t);
+  *n_out = m;
+  if (out_cap < m) return fail(h, WM_ERR_INVALID, "out_cap is smaller than the resampled length");
+  CK(resample_launch(in_dev, n_in, out_dev, m, r.taps, r.sup, r.t, r.T, r.smem, s));
+  return WM_OK;
+}
+
+extern "C" int wm_resample_taps(int32_t orig_hz, int32_t new_hz, float* taps, int32_t* lo, int32_t* n_taps, int64_t cap,
+                                int32_t* info4) {
+  if (!info4) return WM_ERR_INVALID;
+  ResampleTable t;
+  if (!resample_build_table(orig_hz, new_hz, t)) return WM_ERR_INVALID;
+  info4[0] = t.orig; info4[1] = t.nw; info4[2] = t.width; info4[3] = t.max_taps;
+  if (!taps && !lo && !n_taps) return WM_OK;
+  if (!taps || !lo || !n_taps || cap < (int64_t)t.taps.size()) return WM_ERR_INVALID;
+  std::copy(t.taps.begin(), t.taps.end(), taps);
+  for (int p = 0; p < t.nw; ++p) { lo[p] = t.lo[p]; n_taps[p] = t.n[p]; }
+  return WM_OK;
 }
 
 extern "C" int wm_encode_mel_device(wm_handle* h, const float* mel_dev, void* producer_stream) {

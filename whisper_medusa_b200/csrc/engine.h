@@ -47,6 +47,25 @@ cudaError_t mel_forward(const float* pcm, const float* filters /*[201][80]*/, fl
 // mel given by the caller: mel_f32 [80][3000] device -> x_tm
 cudaError_t mel_to_time_major(const float* mel_f32, __half* x_tm, cudaStream_t s, int64_t* n_launch);
 
+// ---- resample.cu ----
+constexpr int kResampleMaxRate = 1 << 20;   // largest rate after dividing both rates by their gcd
+// Polyphase table of one rate pair (host side).  taps [nw][max_taps] row-major, phase p uses taps[p][0 .. n[p]) on
+// padded input columns lo[p] .. lo[p] + n[p] of its block; [dlo, dhi): input reach of output o relative to
+// floor(o * orig / nw).
+struct ResampleTable {
+  int orig = 0, nw = 0, width = 0, max_taps = 0;
+  int64_t dlo = 0, dhi = 0;
+  std::vector<float> taps;
+  std::vector<int> lo, n;
+};
+bool resample_build_table(int orig_hz, int new_hz, ResampleTable& t);
+int64_t resample_out_len(int64_t n_in, const ResampleTable& t);
+// outputs per CTA (0: the input span of 32 outputs does not fit the staging buffer) and its shared-memory bytes
+int resample_block_outputs(const ResampleTable& t, size_t* smem_bytes);
+// taps_dev [max_taps][nw] (the transpose of ResampleTable::taps); sup_dev [nw] {lo - width, n}
+cudaError_t resample_launch(const float* x, int64_t n_in, float* y, int64_t n_out, const float* taps_dev,
+                            const int2* sup_dev, const ResampleTable& t, int T, size_t smem, cudaStream_t s);
+
 // ---- enc_gemm.cu ----
 enum EncEpi { ENC_EPI_BIAS_F16 = 0, ENC_EPI_BIAS_GELU_F16 = 1, ENC_EPI_BIAS_RES_F32 = 2, ENC_EPI_BIAS_GELU_POS_F32 = 3 };
 struct EncGemmArgs {

@@ -13,7 +13,10 @@ scores (`metrics.py` restates jiwer 3.0.3, see there).  Differences, all on the 
   when its backend is available; resampling to 16 kHz uses `torchaudio.functional.resample`;
 * `--frontend engine` (default) feeds the PCM to the engine's own log-mel kernel
   (`generate_from_pcm`); `--frontend hf` computes the features with `WhisperProcessor` on the CPU and
-  calls `generate(input_features)` exactly as the reference does (`eval_whisper_medusa.py:46-65`).
+  calls `generate(input_features)` exactly as the reference does (`eval_whisper_medusa.py:46-65`);
+* `--chunk-length-s S` (S > 0, at most 30) reads each file at its native rate and transcribes it with
+  `model.transcribe(pcm, sampling_rate=sr, chunk_length_s=S)`: recordings of any length, resampled on the GPU
+  (the reference accepts at most 30 s).  The default 0 keeps the path above.
 """
 from __future__ import annotations
 
@@ -29,7 +32,7 @@ from .metrics import compute_cer, compute_wer
 
 SAMPLING_RATE = 16000
 
-__all__ = ["load_audio", "evaluate_rows", "evaluate_model", "main"]
+__all__ = ["load_audio", "load_audio_native", "evaluate_rows", "evaluate_model", "main"]
 
 
 def _read_wav(path: str) -> Tuple[np.ndarray, int]:
@@ -49,15 +52,20 @@ def _read_wav(path: str) -> Tuple[np.ndarray, int]:
     return np.ascontiguousarray(x), sr
 
 
-def load_audio(path: str, sampling_rate: int = SAMPLING_RATE) -> np.ndarray:
-    """Mono float32 PCM at `sampling_rate` (reference eval_whisper_medusa.py:42-46)."""
+def load_audio_native(path: str) -> Tuple[np.ndarray, int]:
+    """Mono float32 PCM at the file's own rate, and that rate."""
     try:
-        x, sr = _read_wav(path)
+        return _read_wav(path)
     except (wave.Error, EOFError):
         import torchaudio   # other containers: whatever backend torchaudio has
 
         t, sr = torchaudio.load(path)
-        x = t[0].numpy().astype(np.float32)
+        return t[0].numpy().astype(np.float32), int(sr)
+
+
+def load_audio(path: str, sampling_rate: int = SAMPLING_RATE) -> np.ndarray:
+    """Mono float32 PCM at `sampling_rate` (reference eval_whisper_medusa.py:42-46)."""
+    x, sr = load_audio_native(path)
     if sr != sampling_rate:
         import torch
         import torchaudio.functional as AF
@@ -92,7 +100,7 @@ def evaluate_rows(rows: Iterable[Dict], transcribe: Callable[[np.ndarray, str], 
 
 def evaluate_model(model_name: str, data_path: str, out_file_path: str, language: str = "en",
                    regulation_start: float = 140, regulation_factor: float = 1.0, frontend: str = "engine",
-                   device: str = "cuda:0"):
+                   device: str = "cuda:0", chunk_length_s: float = 0.0):
     import pandas as pd
     import torch
     from transformers import WhisperProcessor
@@ -104,8 +112,12 @@ def evaluate_model(model_name: str, data_path: str, out_file_path: str, language
     model = WhisperMedusaModel.from_pretrained(model_name).to(device)
     penalty = (regulation_start, regulation_factor) if regulation_factor != 1 else None   # eval_whisper_medusa.py:52-59
 
-    def transcribe(pcm: np.ndarray, lang: str) -> str:
-        if frontend == "hf":
+    def transcribe(pcm, lang: str) -> str:
+        if chunk_length_s > 0:
+            x, sr = pcm
+            out = model.transcribe(x, sampling_rate=sr, chunk_length_s=chunk_length_s, language=lang,
+                                   exponential_decay_length_penalty=penalty)
+        elif frontend == "hf":
             feats = processor(pcm, return_tensors="pt", sampling_rate=SAMPLING_RATE).input_features
             out = model.generate(feats, language=lang, exponential_decay_length_penalty=penalty)
         else:
@@ -113,7 +125,8 @@ def evaluate_model(model_name: str, data_path: str, out_file_path: str, language
         return processor.decode(out[0], skip_special_tokens=True)
 
     with torch.no_grad():
-        wer, cer, table = evaluate_rows(data.to_dict("records"), transcribe, default_language=language)
+        wer, cer, table = evaluate_rows(data.to_dict("records"), transcribe, default_language=language,
+                                        loader=load_audio_native if chunk_length_s > 0 else load_audio)
     logging.info("=======================")
     logging.info(f"WER: {wer}")
     logging.info(f"CER: {cer}")
@@ -134,10 +147,12 @@ def main(argv: Optional[Sequence[str]] = None):
     ap.add_argument("--regulation-factor", type=float, default=1, help="factor for exponential decay (1 = off)")
     ap.add_argument("--frontend", choices=["engine", "hf"], default="engine", help="log-mel on the GPU (engine) or HF features on the CPU")
     ap.add_argument("--device", type=str, default="cuda:0")
+    ap.add_argument("--chunk-length-s", type=float, default=0.0,
+                    help="> 0: long-form transcription in windows of this many seconds (at most 30) at the file's own rate")
     args = ap.parse_args(argv)
     logging.basicConfig(format="%(asctime)s - %(name)s - %(levelname)s - %(message)s", level=logging.INFO)
     evaluate_model(args.model_name, args.data_path, args.out_file_path, args.language, args.regulation_start,
-                   args.regulation_factor, args.frontend, args.device)
+                   args.regulation_factor, args.frontend, args.device, args.chunk_length_s)
 
 
 if __name__ == "__main__":

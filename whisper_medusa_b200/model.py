@@ -10,6 +10,10 @@ Same names, argument meaning and error behaviour as the reference for this path:
   ``NotImplementedError`` (``:1213-1214``); beam search -> ``Exception`` (``:1153-1156``);
 * the returned ``LongTensor[1, n]`` has the prompt and the trailing EOS stripped (``:1929-1973``).
 
+Beyond the reference (which takes 16 kHz clips of at most 30 s): ``transcribe`` takes a recording of any length at any
+integer sampling rate, with the semantics of HF's chunked ASR pipeline (``longform.py``); ``generate_from_pcm`` takes
+``sampling_rate``.  Both resample on the GPU (``csrc/resample.cu``).
+
 There is no PyTorch / CPU fallback: every tensor op of the path runs in the CUDA engine, and the
 constructor raises if the engine library is missing.
 """
@@ -24,9 +28,25 @@ import torch
 
 from . import _lib
 from .config import MedusaConfig, MedusaGenerationConfig
+from .longform import (MAX_WINDOW_SAMPLES, SAMPLE_RATE, Window, WindowResult, merge_windows, plan_windows,
+                       resampled_length, text_ids, window_params)
 from .weights import pack_blob
 
 N_FRAMES = 3000
+
+
+def _rate(sampling_rate) -> int:
+    """A sampling rate as a positive integer (the resampler supports integer rates only)."""
+    if isinstance(sampling_rate, bool) or int(sampling_rate) != sampling_rate or int(sampling_rate) <= 0:
+        raise ValueError(f"sampling_rate must be a positive integer number of Hz, got {sampling_rate!r}")
+    return int(sampling_rate)
+
+
+def _check_recording(audio, sampling_rate) -> None:
+    _rate(sampling_rate)
+    ndim = audio.dim() if isinstance(audio, torch.Tensor) else np.ndim(audio)
+    if ndim != 1:
+        raise ValueError(f"audio must be a 1-D mono recording, got {ndim} dimensions (downmix multi-channel audio first)")
 
 
 class EngineError(RuntimeError):
@@ -107,6 +127,7 @@ class WhisperMedusaModel:
         self._device: Optional[torch.device] = None
         self._wblob_dev: Optional[torch.Tensor] = None
         self.last_trace = GenerateTrace()
+        self.last_windows: List[WindowResult] = []    # per-window results of the last transcribe()
         if len(config.medusa_choices) != config.medusa_num_heads + 1:
             raise ValueError("len(medusa_choices) must be medusa_num_heads + 1")
 
@@ -424,10 +445,21 @@ class WhisperMedusaModel:
             raise NotImplementedError(f"generate() options not implemented by the H100 engine: {unknown}")
 
     def generate_from_pcm(self, pcm: Union[np.ndarray, torch.Tensor], language: Optional[str] = None,
-                          task: Optional[str] = None, temperature=None, **kwargs) -> torch.Tensor:
-        """Same as ``generate`` but takes 16 kHz mono f32 PCM and runs the log-mel frontend on the GPU
-        (what ``WhisperProcessor`` does on the CPU in the reference's caller, eval_whisper_medusa.py:46-51)."""
+                          task: Optional[str] = None, temperature=None, sampling_rate: int = SAMPLE_RATE,
+                          **kwargs) -> torch.Tensor:
+        """Same as ``generate`` but takes mono f32 PCM and runs the log-mel frontend on the GPU
+        (what ``WhisperProcessor`` does on the CPU in the reference's caller, eval_whisper_medusa.py:46-51).
+        ``sampling_rate`` other than 16000 (any positive integer rate): the clip is uploaded and resampled to 16 kHz on
+        the GPU first (``torchaudio.functional.resample`` with its defaults); the 30 s limit applies after resampling."""
         self._require_engine()
+        if _rate(sampling_rate) != SAMPLE_RATE:
+            x = torch.as_tensor(pcm).detach().to(torch.float32).reshape(-1)
+            if resampled_length(x.numel(), _rate(sampling_rate), SAMPLE_RATE) > MAX_WINDOW_SAMPLES:
+                raise NotImplementedError("Longform generation is not supported yet")
+            self._check_unsupported(temperature, None, kwargs)
+            x16 = self._upload_16k(x, sampling_rate)
+            self._encode_window(x16, Window(0, x16.numel(), 0, 0), torch.cuda.current_stream(self._device).cuda_stream)
+            return self._decode(language, task, kwargs, temperature)
         x = torch.as_tensor(pcm).detach().to("cpu", torch.float32).contiguous().reshape(-1)
         if x.numel() > 480000:
             raise NotImplementedError("Longform generation is not supported yet")
@@ -437,6 +469,75 @@ class WhisperMedusaModel:
                "wm_encode_pcm")
         self._check_unsupported(temperature, None, kwargs)
         return self._decode(language, task, kwargs, temperature)
+
+    # ------------------------------------------------------------------ long-form (HF chunked ASR pipeline)
+    def transcribe(self, audio: Union[np.ndarray, torch.Tensor], sampling_rate: int = SAMPLE_RATE,
+                   chunk_length_s: float = 30.0, stride_length_s: Optional[Union[float, Sequence[float]]] = None,
+                   language: Optional[str] = None, task: Optional[str] = None, temperature=None,
+                   **generate_kwargs) -> torch.Tensor:
+        """Transcribe a mono recording of any length at any integer sampling rate; returns ``LongTensor[1, n]``.
+
+        The semantics of HF's ``pipeline("automatic-speech-recognition", chunk_length_s=30)`` without timestamps
+        (``longform.py``): the recording is cut into windows of ``chunk_length_s`` (at most 30 s) overlapping by
+        ``stride_length_s`` on each side (default ``chunk_length_s / 6``), each window is transcribed like a short clip
+        with the same options as ``generate`` (``language=None`` on a multilingual model: each window detects its own
+        language), and the windows' text ids (special ids, all ``>= eos_token_id``, dropped) are merged by the
+        longest-common-sequence rule.
+
+        ``audio``: 1-D f32 samples as a numpy array, a CPU tensor, or a CUDA tensor on the engine's device (used in place,
+        ordered after the current stream).  The recording is uploaded once and, if ``sampling_rate != 16000``, resampled
+        once on the GPU.  Every window's log-mel is computed from the device-resident samples.  Per-window results go
+        to ``self.last_windows``.  An empty recording has no windows and gives ``[1, 0]``."""
+        self._require_engine()
+        params = window_params(chunk_length_s, stride_length_s)
+        _check_recording(audio, sampling_rate)
+        self._check_unsupported(temperature, None, generate_kwargs)
+        x16 = self._upload_16k(audio, sampling_rate)
+        stream = torch.cuda.current_stream(self._device).cuda_stream
+        results = [self._transcribe_window(x16, w, stream, language=language, task=task, temperature=temperature,
+                                           **generate_kwargs)
+                   for w in plan_windows(x16.numel(), *params)]
+        self.last_windows = results
+        merged = merge_windows([text_ids(r.ids, int(self.generation_config.eos_token_id)) for r in results])
+        return torch.tensor([merged], dtype=torch.long, device=self._device)
+
+    def _upload_16k(self, audio, sampling_rate) -> torch.Tensor:
+        """The recording as contiguous f32 16 kHz samples on the engine's device: one upload (none for a CUDA tensor on
+        this device) and, at another rate, one resampling kernel on the current stream."""
+        lib = _lib.load()
+        if isinstance(audio, torch.Tensor) and audio.is_cuda:
+            if audio.device != self._device:
+                raise EngineError(f"audio is on {audio.device}, the engine on {self._device}")
+            x = audio.detach().to(torch.float32).reshape(-1).contiguous()
+        else:
+            x = torch.as_tensor(audio).detach().to(torch.float32).reshape(-1).contiguous().to(self._device)
+        sr = _rate(sampling_rate)
+        if sr == SAMPLE_RATE or x.numel() == 0:
+            return x
+        n_out = resampled_length(x.numel(), sr, SAMPLE_RATE)
+        y = torch.empty(n_out, dtype=torch.float32, device=self._device)
+        got = C.c_int64(0)
+        stream = torch.cuda.current_stream(self._device).cuda_stream
+        _check(lib, self._handle,
+               lib.wm_resample(self._handle, C.c_void_p(x.data_ptr()), x.numel(), sr, SAMPLE_RATE, C.c_void_p(y.data_ptr()),
+                               n_out, C.byref(got), C.c_void_p(stream)), "wm_resample")
+        if got.value != n_out:
+            raise EngineError(f"wm_resample produced {got.value} samples, expected {n_out}")
+        return y
+
+    def _encode_window(self, x16: torch.Tensor, w: Window, producer_stream: int) -> None:
+        """Log-mel + encoder of samples ``w.start:w.end`` of a device-resident 16 kHz recording."""
+        lib = _lib.load()
+        ptr = x16.data_ptr() + w.start * x16.element_size()
+        _check(lib, self._handle,
+               lib.wm_encode_pcm_device(self._handle, C.c_void_p(ptr), int(w.end - w.start), C.c_void_p(producer_stream)),
+               "wm_encode_pcm_device")
+
+    def _transcribe_window(self, x16: torch.Tensor, w: Window, producer_stream: int, language=None, task=None,
+                           temperature=None, **kwargs) -> WindowResult:
+        self._encode_window(x16, w, producer_stream)
+        ids = self._decode(language, task, kwargs, temperature)[0].tolist()
+        return WindowResult(w, ids, self.last_trace)
 
     def _decode(self, language, task, kwargs, temperature, generation_config=None) -> torch.Tensor:
         g = generation_config if generation_config is not None else self.generation_config

@@ -54,6 +54,7 @@ class StreamGroup:
         self.config = config
         self.device = torch.device("cuda", index)
         self.last_traces: List[GenerateTrace] = []
+        self.last_windows: List[list] = []
         self.last_wall_s = 0.0
         self.last_decode_phase_s = 0.0
 
@@ -110,6 +111,37 @@ class StreamGroup:
         """16 kHz mono PCM clips (each <= 30 s) -> one ``LongTensor[1, n_i]`` per clip (arguments of
         ``WhisperMedusaModel.generate_from_pcm``)."""
         return self._run(clips, lambda m, x, kw: m.generate_from_pcm(x, **kw), kwargs)
+
+    def transcribe(self, recordings, sampling_rate: Union[int, Sequence[int]] = 16000, chunk_length_s: float = 30.0,
+                   stride_length_s=None, **kwargs) -> List[torch.Tensor]:
+        """Long-form ``WhisperMedusaModel.transcribe`` of one recording or a list of them (``sampling_rate``: one rate
+        for all, or one per recording) -> one ``LongTensor[1, n_i]`` per recording.
+
+        Each recording is uploaded and resampled once into a device buffer that every engine reads; the windows of all
+        recordings go into one work queue, so they decode concurrently on the S engines, and each recording's windows
+        are merged in order.  The results equal ``model.transcribe`` of each recording.  Per-window results:
+        ``self.last_windows[i]`` for recording i."""
+        from .longform import merge_windows, plan_windows, text_ids, window_params
+        from .model import _check_recording
+
+        recs = [recordings] if isinstance(recordings, (np.ndarray, torch.Tensor)) else list(recordings)
+        rates = list(sampling_rate) if isinstance(sampling_rate, (list, tuple)) else [sampling_rate] * len(recs)
+        if len(rates) != len(recs):
+            raise ValueError(f"{len(rates)} sampling rates for {len(recs)} recordings")
+        params = window_params(chunk_length_s, stride_length_s)
+        for r, sr in zip(recs, rates):
+            _check_recording(r, sr)
+        lead = self.models[0]
+        lead._check_unsupported(kwargs.get("temperature"), None,
+                                {k: v for k, v in kwargs.items() if k not in ("language", "task", "temperature")})
+        x16 = [lead._upload_16k(r, sr) for r, sr in zip(recs, rates)]
+        stream = torch.cuda.current_stream(self.device).cuda_stream     # every window's encode is ordered after it
+        items = [(i, w) for i, x in enumerate(x16) for w in plan_windows(x.numel(), *params)]
+        results = self._run(items, lambda m, it, kw: m._transcribe_window(x16[it[0]], it[1], stream, **kw), kwargs)
+        eos = int(lead.generation_config.eos_token_id)
+        self.last_windows = [[res for (i, _), res in zip(items, results) if i == k] for k in range(len(recs))]
+        return [torch.tensor([merge_windows([text_ids(r.ids, eos) for r in ws])], dtype=torch.long, device=self.device)
+                for ws in self.last_windows]
 
     def generate(self, input_features: torch.Tensor, **kwargs) -> List[torch.Tensor]:
         """``input_features [B, 80, 3000]`` with any B (the batch dimension the reference refuses, model.py:1451):
