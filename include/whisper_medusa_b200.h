@@ -152,6 +152,9 @@ int wm_last_logits(wm_handle* h, int32_t which, float* out);
 double wm_last_ms(wm_handle* h, int32_t what);
 /* Number of kernel launches issued by the last wm_encode_* (what=1) / wm_generate (what=2). */
 int64_t wm_last_launches(wm_handle* h, int32_t what);
+/* CTAs per thread-block cluster of the persistent ring kernel: 2 when its grid is the whole GPU and the device can hold
+ * all of those 2-CTA clusters at once (activation rows are then multicast to both CTAs of a cluster), else 1. */
+int wm_decode_cluster(wm_handle* h);
 /* Decode execution mode: 2 (DEFAULT) = one persistent cooperative kernel per speculative iteration with the
  * shared-memory weight ring (bulk-async prefetch across barriers; the product path); 1 = the same without the
  * ring (grid barriers only); 0 = CUDA graphs of stage kernels (debug / per-stage profiling, and the automatic

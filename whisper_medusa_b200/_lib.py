@@ -62,6 +62,7 @@ SYMBOLS = {
     "wm_last_logits": (C.c_int, [C.c_void_p, C.c_int32, _P(C.c_float)]),
     "wm_last_ms": (C.c_double, [C.c_void_p, C.c_int32]),
     "wm_last_launches": (C.c_int64, [C.c_void_p, C.c_int32]),
+    "wm_decode_cluster": (C.c_int, [C.c_void_p]),
     "wm_set_decode_mode": (C.c_int, [C.c_void_p, C.c_int32]),
     "wm_weights_device_ptr": (C.c_void_p, [C.c_void_p]),
     "wm_enc_gemm_tile": (C.c_int, [C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, _P(C.c_int32)]),

@@ -66,8 +66,11 @@ struct alignas(16) CtaStage {
                             //    LayerNorm stages: X = xg, the statistics come from the fp32 rows of x)
   int out_split;            // 1: the epilogue writes `out` in that format (the consumer is a presplit stage)
   float* out_gx;            // residual epilogues: also write nx_g o out in that format here (the next stage's xg)
-  int pad_[2];
+  int x_role;               // staging of X in a 2-CTA cluster (XR_*): the host sets issue / receive only where both CTAs
+                            //    of the pair stage the same rows (same X, x_ld, T rule, and both n_rows > 0)
+  int pad_;
 };
+enum XRole { XR_OWN = 0, XR_ISSUE = 1, XR_RECEIVE = 2 };   // own copies / multicast to both CTAs / wait for the peer's multicast
 static_assert(sizeof(CtaStage) == 128, "CtaStage must be one 128-byte line");
 
 // Barrier over the WM_DEC_THREADS compute threads of a decode CTA.  The persistent ring kernel has

@@ -1403,8 +1403,16 @@ __device__ __forceinline__ unsigned int ld_relaxed_u32(const unsigned int* p) {
 template <bool ACQUIRE>
 __device__ __forceinline__ unsigned int grid_barrier_step(unsigned int* bar, unsigned int epoch, int ncta) {
   // the ring kernel's consumers fetch activations with bulk async copies: order this thread's generic-proxy
-  // global writes before async-proxy reads that follow the barrier
-  if (!ACQUIRE) asm volatile("fence.proxy.async.global;" ::: "memory");
+  // global writes before async-proxy reads that follow the barrier.  In a 2-CTA cluster the peer multicasts the next
+  // stage's rows into this CTA's scratch region (also used by the attention stages and the split passes) as soon as
+  // the barrier opens: this thread's generic accesses of its shared memory must be ordered before those async writes
+  // too.  Unclustered launches skip that fence (every CTA then writes only its own shared memory, after its own fence).
+  if (!ACQUIRE) {
+    asm volatile("fence.proxy.async.global;" ::: "memory");
+    uint32_t ncl;
+    asm volatile("mov.u32 %0, %%cluster_nctarank;" : "=r"(ncl));
+    if (ncl > 1) asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+  }
   cta_sync();
   if (threadIdx.x == 0) {
     const unsigned int target = (unsigned int)ncta * (epoch + 1u);
@@ -1562,8 +1570,9 @@ cudaError_t dec_fold_layernorms(const DecModel& hm, int n_dec, float2* out, cuda
   return cudaGetLastError();
 }
 
-// Resolved stage records of the ring kernel: tab[ip * ncta + cta] (see CtaStage in common.cuh).
-void dec_build_stage_table(const DecModel& hm, const float2* ln_fold, int ncta, std::vector<CtaStage>& tab) {
+// Resolved stage records of the ring kernel: tab[ip * ncta + cta] (see CtaStage in common.cuh).  `cluster`: CTAs per
+// cluster of the launch the table is for (dec_ring_cluster_size).
+void dec_build_stage_table(const DecModel& hm, const float2* ln_fold, int ncta, int cluster, std::vector<CtaStage>& tab) {
   std::vector<int> flat;
   int poff[4];
   dec_build_program(hm.n_layers, hm.has_block, flat, poff);
@@ -1634,6 +1643,17 @@ void dec_build_stage_table(const DecModel& hm, const float2* ln_fold, int ncta, 
         if (ps == ST_OPROJ || ps == ST_CROSS_O || ps == ST_FC2) { c.presplit = 1; c.X = hm.xg; }
       }
     }
+    // 2-CTA clusters (CTAs 2i, 2i + 1): one multicast copy of X for both where they stage the same rows.  Both must have
+    // rows: a CTA without rows returns before staging, and the peer's complete_tx would then shift its xbar phase.
+    if (cluster == 2 && is_gemm_stage(stage))
+      for (int cta = 0; cta + 1 < ncta; cta += 2) {
+        CtaStage& a = tab[(size_t)ip * ncta + cta];
+        CtaStage& b = tab[(size_t)ip * ncta + cta + 1];
+        if (a.n_rows > 0 && b.n_rows > 0 && a.X == b.X && a.x_ld == b.x_ld && a.x_rows_fixed == b.x_rows_fixed) {
+          a.x_role = XR_ISSUE;
+          b.x_role = XR_RECEIVE;
+        }
+      }
   }
 }
 
@@ -1644,16 +1664,59 @@ cudaError_t dec_relayout_cross_kv(const __half* kv, __half* ck, __half* cv, int 
   return cudaGetLastError();
 }
 
-cudaError_t dec_launch_iteration_ring(const DecModel* dm, const DecHostInfo& hi, bool profile, cudaStream_t s) {
-  void* args[] = {(void*)&dm};
-  void* fn = nullptr;
-  switch (hi.d) {
-#define WM_CASE(DD) case DD: fn = profile ? (void*)dec_iteration_ring_kernel<DD, true> : (void*)dec_iteration_ring_kernel<DD, false>; break;
+static void* ring_kernel_fn(int d, bool profile) {
+  switch (d) {
+#define WM_CASE(DD) case DD: return profile ? (void*)dec_iteration_ring_kernel<DD, true> : (void*)dec_iteration_ring_kernel<DD, false>;
     WM_RING_WIDTHS(WM_CASE)
 #undef WM_CASE
-    default: return cudaErrorInvalidValue;
+    default: return nullptr;
   }
-  return cudaLaunchCooperativeKernel(fn, dim3(hi.n_sm), dim3(WM_RING_THREADS), args, hi.smem_ring, s);
+}
+
+// Cooperative launch (the grid barrier needs every CTA resident), as clusters of hi.cluster CTAs along x.
+cudaError_t dec_launch_iteration_ring(const DecModel* dm, const DecHostInfo& hi, bool profile, cudaStream_t s) {
+  void* fn = ring_kernel_fn(hi.d, profile);
+  if (!fn) return cudaErrorInvalidValue;
+  void* args[] = {(void*)&dm};
+  cudaLaunchAttribute attr[2];
+  attr[0].id = cudaLaunchAttributeCooperative;
+  attr[0].val.cooperative = 1;
+  attr[1].id = cudaLaunchAttributeClusterDimension;
+  attr[1].val.clusterDim.x = (unsigned)hi.cluster;
+  attr[1].val.clusterDim.y = 1;
+  attr[1].val.clusterDim.z = 1;
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(hi.n_sm);
+  cfg.blockDim = dim3(WM_RING_THREADS);
+  cfg.dynamicSmemBytes = hi.smem_ring;
+  cfg.stream = s;
+  cfg.attrs = attr;
+  cfg.numAttrs = hi.cluster > 1 ? 2 : 1;
+  return cudaLaunchKernelExC(&cfg, fn, args);
+}
+
+// CTAs per cluster of the ring kernel on a grid of hi.n_sm CTAs: 2 when the grid is the whole device (an even number of
+// SMs) and the device can hold n_sm / 2 such clusters at once, else 1.  Needs dec_configure first (shared-memory size).
+int dec_ring_cluster_size(const DecHostInfo& hi, int n_sm) {
+  void* fn = ring_kernel_fn(hi.d, false);
+  if (!fn || hi.n_sm != n_sm || n_sm % 2 != 0) return 1;
+  cudaLaunchAttribute attr;
+  attr.id = cudaLaunchAttributeClusterDimension;
+  attr.val.clusterDim.x = 2;
+  attr.val.clusterDim.y = 1;
+  attr.val.clusterDim.z = 1;
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(n_sm);
+  cfg.blockDim = dim3(WM_RING_THREADS);
+  cfg.dynamicSmemBytes = hi.smem_ring;
+  cfg.attrs = &attr;
+  cfg.numAttrs = 1;
+  int n = 0;
+  if (cudaOccupancyMaxActiveClusters(&n, fn, &cfg) != cudaSuccess) {
+    (void)cudaGetLastError();
+    return 1;
+  }
+  return n >= n_sm / 2 ? 2 : 1;
 }
 
 size_t dec_smem_bytes(int d, int ffn) {

@@ -30,6 +30,13 @@
 // segment partials go to a global scratch and the CTA that arrives last for a row block folds
 // them in segment order (deterministic) and runs the epilogue.
 //
+// On the whole GPU the kernel runs as 2-CTA clusters (CTAs 2i, 2i+1; still a cooperative launch:
+// the grid barrier needs every CTA resident).  Every CTA of a GEMM stage stages the same activation
+// rows, so where both CTAs of a pair have rows, the even one multicasts them into both CTAs' shared
+// memory (one L2 read per pair; CtaStage::x_role) and the odd one only waits for them.  The kernel
+// reads the cluster size at run time: partial grids launch unclustered and every CTA copies its own
+// rows.
+//
 // Ring geometry: a "chunk" = up to 16 weight rows x d columns (fp16), row stride d*2 + 64 B
 // (bank-conflict-free LDS.128 of the B fragments); WM_RING_G chunks are resident; chunks are
 // consumed in program order.
@@ -70,6 +77,22 @@ __device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t by
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(smem_u32(dst)),
                "l"(src), "r"(bytes), "r"(smem_u32(bar))
                : "memory");
+}
+// the same copy into the same CTA-relative offsets (dst and mbarrier) of every CTA of the cluster in cta_mask
+__device__ __forceinline__ void bulk_g2s_multicast(void* dst, const void* src, uint32_t bytes, uint64_t* bar, uint16_t cta_mask) {
+  asm volatile(
+      "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1], %2, [%3], %4;" ::"r"(
+          smem_u32(dst)),
+      "l"(src), "r"(bytes), "r"(smem_u32(bar)), "h"(cta_mask)
+      : "memory");
+}
+__device__ __forceinline__ uint32_t cluster_ncta() {
+  uint32_t n;
+  asm volatile("mov.u32 %0, %%cluster_nctarank;" : "=r"(n));
+  return n;
+}
+__device__ __forceinline__ void cluster_sync_all() {
+  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
 __device__ __forceinline__ unsigned long long global_timer_ns() {
   unsigned long long t;
@@ -113,6 +136,8 @@ __host__ __device__ __forceinline__ void cta_rows(int N, int part, int nparts, i
 
 // Work of one CTA in a GEMM stage: rows [n_begin, n_begin + n_rows) of W, k segment `seg` of `segs`
 // (segs > 1 <=> K > d: the stage is split along K over CTAs; `block` = row block shared by `segs` CTAs).
+// Consecutive CTAs take consecutive row blocks of ONE segment, so the two CTAs of a cluster read the same k slice of
+// the activations and can share one multicast copy of it.
 struct GemmWork { int n_begin, n_rows, seg, segs, block; };
 __host__ __device__ __forceinline__ GemmWork gemm_work(int N, int K, int d, int cta, int ncta) {
   GemmWork w;
@@ -124,8 +149,8 @@ __host__ __device__ __forceinline__ GemmWork gemm_work(int N, int K, int d, int 
   }
   const int nb = ncta / w.segs;   // host guarantees nb >= 1
   if (cta >= nb * w.segs) { w.n_begin = 0; w.n_rows = 0; w.seg = 0; w.block = 0; return w; }
-  w.block = cta / w.segs;
-  w.seg = cta - w.block * w.segs;
+  w.seg = cta / nb;
+  w.block = cta - w.seg * nb;
   cta_rows(N, w.block, nb, w.n_begin, w.n_rows);
   return w;
 }
@@ -313,13 +338,21 @@ __device__ __forceinline__ void stage_gemm_ring(RingState& rs, unsigned char* sm
     pr[11] = mbar_try_wait(full + rs.slot, rs.par) ? 1000ull : 0ull;   // weights already here?
   }
   // ---- X rows: global (L2) -> shared, one bulk copy per row ----
+  // In a 2-CTA cluster whose CTAs stage the same rows, the issuing CTA multicasts each row into the same offsets of both
+  // CTAs (one L2 read per pair) and signals both xbars; the receiving CTA only arms its own xbar for the same bytes.  A
+  // complete_tx that reaches the receiver's xbar before its arrival cannot finish the phase (the arrival is pending).
   if (warp == 0) {
+    const int role = sd->x_role;
     if (lane == 0) {
       asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // earlier generic accesses of the buffer vs async writes
       mbar_expect_tx(xbar, (uint32_t)(T * D * 4));
     }
     __syncwarp();
-    if (lane < T) bulk_g2s(xb + (size_t)lane * G::XS, sd->X + (size_t)lane * sd->x_ld, (uint32_t)(D * 4), xbar);
+    if (lane < T) {
+      if (role == XR_OWN) bulk_g2s(xb + (size_t)lane * G::XS, sd->X + (size_t)lane * sd->x_ld, (uint32_t)(D * 4), xbar);
+      else if (role == XR_ISSUE)
+        bulk_g2s_multicast(xb + (size_t)lane * G::XS, sd->X + (size_t)lane * sd->x_ld, (uint32_t)(D * 4), xbar, 0x3);
+    }
   } else if (warp == 1) {
     // this CTA's bias slice of the NEXT GEMM stage -> L2 (biases are cold: 2 GB of weights pass through L2 per iteration)
     if (lane < sd->pf_bias_lines) prefetch_l2(reinterpret_cast<const unsigned char*>(sd->pf_bias) + (size_t)lane * 128);
@@ -629,6 +662,10 @@ dec_iteration_ring_kernel(const DecModel* __restrict__ gm) {
     for (int i = threadIdx.x; i < (int)((sizeof(DecModel) + 15) / 16); i += WM_RING_THREADS) dst[i] = src[i];
   }
   __syncthreads();   // the only full-CTA barrier: after it the producer warp goes its own way
+  // Clustered launch: the peer multicasts into this CTA's xbar as soon as its first GEMM stage begins, and with
+  // need_a = 0 that is the HEADS stage, with no grid barrier before it.  So every thread of both CTAs passes one cluster
+  // barrier after the mbarrier initialisation (released to the cluster above) and before any stage runs.
+  if (cluster_ncta() > 1) cluster_sync_all();
   const DecModel* m = sm;
 
   if (warp == WM_DEC_THREADS / 32) {
@@ -691,6 +728,9 @@ dec_iteration_ring_kernel(const DecModel* __restrict__ gm) {
     epoch = grid_barrier_step<false>(m->bar, epoch, ncta);
     if (prof) pr[2] = global_timer_ns();
   }
+  // Every instruction ends in a grid barrier, and a CTA arrives there only after its xbar phase of the stage completed,
+  // i.e. after every multicast byte addressed to it landed.  So past the last barrier no multicast is in flight and
+  // nothing targets the peer's shared memory: the CTAs of a cluster may exit independently.
   if (blockIdx.x == 0 && threadIdx.x == 0) m->bar[2] = epoch;
 }
 

@@ -342,6 +342,7 @@ extern "C" int wm_create(const wm_config* cfg, int device, wm_handle** out) {
   h->hi.smem = dec_smem_bytes((int)d, (int)f);
   h->hi.smem_ring = dec_ring_smem_bytes((int)d);
   CK(dec_configure((int)d, h->hi.smem, h->hi.smem_ring));
+  h->hi.cluster = dec_ring_cluster_size(h->hi, h->n_sm);
   // product path by default: one persistent ring-kernel launch per speculative iteration.  Decoder widths the ring
   // kernel is not instantiated for (WM_RING_WIDTHS) fall back to the stage-kernel graphs.
   h->decode_mode = h->hi.smem_ring ? 2 : 0;
@@ -463,7 +464,7 @@ static int bind_weights(wm_handle* h) {
     m.chunk_tab = h->chunk_tab;
     m.chunk_off = h->chunk_off;
     std::vector<CtaStage> stab;
-    dec_build_stage_table(m, h->ln_fold, h->n_cta, stab);
+    dec_build_stage_table(m, h->ln_fold, h->n_cta, h->hi.cluster, stab);
     if (h->stage_tab) { cudaFree(h->stage_tab); h->stage_tab = nullptr; }
     CK(cudaMalloc((void**)&h->stage_tab, stab.size() * sizeof(CtaStage)));
     CK(cudaMemcpy(h->stage_tab, stab.data(), stab.size() * sizeof(CtaStage), cudaMemcpyHostToDevice));
@@ -1020,6 +1021,7 @@ extern "C" int64_t wm_last_launches(wm_handle* h, int32_t what) {
   if (what == 2) return h->launches[2];
   return -1;
 }
+extern "C" int wm_decode_cluster(wm_handle* h) { return h ? h->hi.cluster : 0; }
 extern "C" int wm_set_option(wm_handle* h, const char* key, int32_t value) {
   if (!h || !key) return WM_ERR_INVALID;
   const std::string k(key);
@@ -1039,6 +1041,7 @@ extern "C" int wm_set_option(wm_handle* h, const char* key, int32_t value) {
     CK(cudaStreamSynchronize(h->stream));
     h->n_cta = value;
     h->hi.n_sm = value;
+    h->hi.cluster = dec_ring_cluster_size(h->hi, h->n_sm);
     set_decode_split(h);
     for (auto& kv : h->graph_a) cudaGraphExecDestroy(kv.second);
     h->graph_a.clear();

@@ -17,6 +17,7 @@ struct DecHostInfo {
   int d;
   size_t smem;
   size_t smem_ring;
+  int cluster = 1; // CTAs per cluster of the ring kernel (1 or 2, dec_ring_cluster_size)
 };
 
 // ---- decode.cu ----
@@ -33,8 +34,9 @@ cudaError_t dec_relayout_cross_kv(const __half* kv, __half* ck, __half* cv, int 
 size_t dec_ln_fold_len(int n_dec, int d, int ffn);
 cudaError_t dec_fold_layernorms(const DecModel& hm, int n_dec, float2* out, cudaStream_t s);
 struct CtaStage;
-void dec_build_stage_table(const DecModel& hm, const float2* ln_fold, int ncta, std::vector<CtaStage>& tab);
+void dec_build_stage_table(const DecModel& hm, const float2* ln_fold, int ncta, int cluster, std::vector<CtaStage>& tab);
 cudaError_t dec_launch_iteration_ring(const DecModel* dm, const DecHostInfo& hi, bool profile, cudaStream_t s);
+int dec_ring_cluster_size(const DecHostInfo& hi, int n_sm);
 // phase: 0 = sweep A over T uncached rows, 1 = tail (candidates), 2 = verify sweep + accept
 cudaError_t dec_enqueue_phase(const DecModel* dm, const DecHostInfo& hi, int phase, int T, cudaStream_t s, int64_t* n_launch);
 cudaError_t dec_launch_iteration(const DecModel* dm, const DecHostInfo& hi, cudaStream_t s);

@@ -111,6 +111,7 @@ class GenerateTrace:
         self.n_new_tokens = 0                 # effective decoded tokens (up to and incl. first EOS)
         self.ms_mel = self.ms_encoder = self.ms_decode = 0.0
         self.launches_encode = self.launches_decode = 0
+        self.cluster_decode = 1                # CTAs per cluster of the persistent ring kernel
 
 
 class WhisperMedusaModel:
@@ -365,6 +366,7 @@ class WhisperMedusaModel:
         tr.ms_mel, tr.ms_encoder, tr.ms_decode = (lib.wm_last_ms(self._handle, i) for i in range(3))
         tr.launches_encode = lib.wm_last_launches(self._handle, 1)
         tr.launches_decode = lib.wm_last_launches(self._handle, 2)
+        tr.cluster_decode = lib.wm_decode_cluster(self._handle)
         return tr
 
     @staticmethod
