@@ -145,7 +145,9 @@ int wm_forward(wm_handle* h, const int32_t* ids, int32_t n_ids, float* out);
 int wm_get_mel(wm_handle* h, float* out /* [n_mels][3000] */);
 int wm_get_encoder_out(wm_handle* h, float* out /* [max_source_positions][d_model] */);
 /* Raw (pre-processor) logits of the last executed iteration: which = 0 pass A ([K+1][V], rows =
- * heads at the last position), 1 = pass B ([K+1][V], rows = tree positions). */
+ * heads at the last position), 1 = pass B ([K+1][V], rows = the first K+1 tree positions), 2 = pass B of every
+ * verify row ([n_tree][V], rows = tree nodes level by level, the order of the reference's tree_indices; n_tree = K+1
+ * for a chain, up to 16 for a branching medusa_choices tree). */
 int wm_last_logits(wm_handle* h, int32_t which, float* out);
 /* Device time (CUDA events on the handle's stream) of the last call: 0 = mel, 1 = encoder
  * (+cross K/V), 2 = decode loop.  Milliseconds. */

@@ -49,16 +49,29 @@ def check_logits(engine, ref64, case, what, ref32=None, bar=None):
     return err
 
 
-def decode_logits(cfg, sd, enc, kw, n_iters, dtype=torch.float64, threads=16):
+def decode_logits(cfg, sd, enc, kw, n_iters, dtype=torch.float64, threads=16, prompt=None, begin_index=None,
+                  prompt_len=None, tree_attention=False):
     """Oracle decode loop (engine regime, working dtype ``dtype``) started from the given encoder states; the trace
-    holds the raw pass-A / pass-B logits of the first ``n_iters`` iterations."""
+    holds the raw pass-A / pass-B logits of the first ``n_iters`` iterations.
+
+    ``prompt``: decoder ids to start from (default: the model's start tokens).  Given an engine's history up to the start
+    of iteration n together with ``begin_index`` / ``prompt_len`` of the ORIGINAL prompt (so that the begin-suppress and
+    length-penalty processors see what they saw in the real run), one iteration of this loop gives the logits and the
+    tokens of iteration n of the real run: pass A recomputes every cached row from the ids alone, which for chains and
+    for ``tree_attention=True`` is what the real loop's cache holds (tests/test_oracle_history_prompt.py)."""
     torch.set_num_threads(threads)
     w = W.RefWeights(sd, dtype)
-    prompt = M.init_tokens(cfg, kw.get("language"))
+    if prompt is None:
+        prompt = M.init_tokens(cfg, kw.get("language"))
     extra = {k: kw[k] for k in ("posterior_alpha", "posterior_threshold") if k in kw}
+    if begin_index is not None:
+        extra["begin_index"] = int(begin_index)
+    if prompt_len is not None:
+        extra["prompt_len"] = int(prompt_len)
     gp = M.gen_params(cfg, prompt, kw.get("exponential_decay_length_penalty"), kw["max_length"],
                       temperature=kw.get("medusa_temperature", 1.0), **extra)
-    return M.medusa_greedy_search(w, cfg, enc, prompt, gp, "engine", capture_logits=n_iters, max_iters=n_iters)
+    return M.medusa_greedy_search(w, cfg, enc, [int(t) for t in prompt], gp, "engine", capture_logits=n_iters,
+                                  max_iters=n_iters, tree_attention=tree_attention)
 
 
 def forward_logits(cfg, sd, enc, ids, dtype=torch.float64):

@@ -1008,9 +1008,10 @@ extern "C" int wm_get_encoder_out(wm_handle* h, float* out) {
   return WM_OK;
 }
 extern "C" int wm_last_logits(wm_handle* h, int32_t which, float* out) {
-  if (!h || !out || which < 0 || which > 1) return WM_ERR_INVALID;
+  if (!h || !out || which < 0 || which > 2) return WM_ERR_INVALID;
   CK(cudaSetDevice(h->device));
-  const size_t n = (size_t)(h->cfg.medusa_num_heads + 1) * h->cfg.vocab_size;
+  const size_t rows = (which == 2) ? (size_t)h->hm.n_tree : (size_t)(h->cfg.medusa_num_heads + 1);
+  const size_t n = rows * h->cfg.vocab_size;
   CK(cudaMemcpy(out, which == 0 ? h->hm.logits_a : h->hm.logits_b, n * sizeof(float), cudaMemcpyDeviceToHost));
   return WM_OK;
 }

@@ -619,8 +619,17 @@ class WhisperMedusaModel:
 
     # ------------------------------------------------------------------ parity taps
     def last_logits(self, which: int) -> torch.Tensor:
+        """Raw logits of the last iteration: 0 = pass A ``[K+1, V]`` (every head at the newest position), 1 = the first
+        K+1 verify rows ``[K+1, V]``, 2 = every verify row ``[n_tree, V]`` (tree nodes level by level)."""
         self._require_engine()
-        n = (self.config.medusa_num_heads + 1, self.config.vocab_size)
+        rows = self.config.medusa_num_heads + 1
+        if which == 2:
+            rows = 0
+            level = 1
+            for c in self.config.medusa_choices:
+                level *= int(c)
+                rows += level
+        n = (rows, self.config.vocab_size)
         out = torch.empty(n, dtype=torch.float32)
         lib = _lib.load()
         _check(lib, self._handle, lib.wm_last_logits(self._handle, which, C.cast(out.data_ptr(), C.POINTER(C.c_float))),
