@@ -24,10 +24,10 @@ of the reference model: for that part parity is "unpinned" (see DESIGN.md).
     cross-attention K/V caches).  Token-id parity is asserted against this regime; logits
     closeness is asserted against both.
 
-The decoder side (``decoder_forward``, ``medusa_logits`` and the loop in ``medusa_ref.py``) also
-runs in fp64 (``RefWeights(sd, dtype=torch.float64)``): the engine regime then still rounds the
-K/V caches to fp16 and widens them back, and everything else is fp64.  The fp32 results are
-unchanged by a bit.
+Everything also runs in fp64: ``RefWeights(sd, dtype=torch.float64)`` for the encoder, the decoder side
+(``decoder_forward``, ``medusa_logits`` and the loop in ``medusa_ref.py``), and
+``log_mel_spectrogram(pcm, torch.float64)`` for the frontend.  The engine regime then still rounds to fp16
+where the engine does and widens back, and everything else is fp64.  The fp32 results are unchanged by a bit.
 """
 from __future__ import annotations
 
@@ -75,8 +75,8 @@ def _mel_to_hz_slaney(m):
 
 
 def mel_filter_bank(n_freq: int = 201, n_mels: int = 80, fmin: float = 0.0, fmax: float = 8000.0,
-                    sr: int = SAMPLE_RATE) -> np.ndarray:
-    """Slaney-normalised triangular filters ``[n_freq, n_mels]``.
+                    sr: int = SAMPLE_RATE, dtype=np.float32) -> np.ndarray:
+    """Slaney-normalised triangular filters ``[n_freq, n_mels]`` (computed in fp64, returned as ``dtype``).
 
     Follows HF ``audio_utils.py:mel_filter_bank`` (norm="slaney", mel_scale="slaney") as
     called from HF ``feature_extraction_whisper.py:95-103``.
@@ -91,7 +91,7 @@ def mel_filter_bank(n_freq: int = 201, n_mels: int = 80, fmin: float = 0.0, fmax
     fb = np.maximum(0.0, np.minimum(down, up))
     enorm = 2.0 / (filter_freqs[2 : n_mels + 2] - filter_freqs[:n_mels])
     fb *= np.expand_dims(enorm, 0)
-    return fb.astype(np.float32)
+    return fb.astype(dtype)
 
 
 def pad_or_trim(pcm: np.ndarray) -> np.ndarray:
@@ -105,23 +105,24 @@ def pad_or_trim(pcm: np.ndarray) -> np.ndarray:
     return out
 
 
-def log_mel_spectrogram(pcm: np.ndarray) -> np.ndarray:
-    """f32 PCM -> ``[80, 3000]`` f32 log-mel.
+def log_mel_spectrogram(pcm: np.ndarray, dtype: torch.dtype = torch.float32) -> np.ndarray:
+    """f32 PCM -> ``[80, 3000]`` log-mel in ``dtype``.
 
     Follows HF ``feature_extraction_whisper.py:135-164`` (``_torch_extract_fbank_features``):
     hann(400) STFT (center, reflect pad), hop 160, |.|^2, drop last frame, mel, log10 with
-    clamp 1e-10, floor at global max - 8, (x + 4) / 4.
+    clamp 1e-10, floor at global max - 8, (x + 4) / 4.  ``dtype=torch.float64``: window, STFT, filters, log10
+    and floor in fp64 (the f32 samples are widened exactly), a reference for the fp32 frontends.
     """
-    wav = torch.from_numpy(pad_or_trim(pcm))
-    window = torch.hann_window(N_FFT)
+    wav = torch.from_numpy(pad_or_trim(pcm)).to(dtype)
+    window = torch.hann_window(N_FFT, dtype=dtype)
     stft = torch.stft(wav, N_FFT, HOP, window=window, return_complex=True)
     mag = stft[..., :-1].abs() ** 2
-    fb = torch.from_numpy(mel_filter_bank())
+    fb = torch.from_numpy(mel_filter_bank(dtype=np.float64 if dtype == torch.float64 else np.float32))
     mel = fb.T @ mag
     log_spec = torch.clamp(mel, min=1e-10).log10()
     log_spec = torch.maximum(log_spec, log_spec.max() - 8.0)
     log_spec = (log_spec + 4.0) / 4.0
-    return log_spec.numpy().astype(np.float32)
+    return log_spec.numpy().astype(np.float64 if dtype == torch.float64 else np.float32)
 
 
 # --------------------------------------------------------------------------------------
@@ -130,14 +131,19 @@ def log_mel_spectrogram(pcm: np.ndarray) -> np.ndarray:
 class RefWeights:
     """View of an fp16 checkpoint state dict (reference key layout, SURVEY.md 3.1) in the working dtype.
 
-    ``dtype`` is the dtype every decoder-side function computes in: fp32 (default, the reference's numerics) or
-    fp64 (an independent high-precision reference for the engine's decode path; the engine regime still rounds the
-    K/V caches to fp16 and widens them back).  The encoder is fp32-only."""
+    ``dtype`` is the dtype every function computes in: fp32 (default, the reference's numerics) or fp64 (an
+    independent high-precision reference for the engine; the engine regime still rounds to fp16 at the engine's
+    rounding points and widens back)."""
 
     def __init__(self, state_dict: Dict[str, torch.Tensor], dtype: torch.dtype = torch.float32):
         self.dtype = dtype
         self.sd = {k: v.detach().to(dtype) for k, v in state_dict.items()}
         self.ln_probe = None     # optional callable(prefix, x): sees every LayerNorm input (statistics in tests)
+        # optional callable(name, t): sees every encoder fp16 rounding point before it rounds ("mel", "conv1",
+        # "layers.{i}.ln1" / "q" / "k" / "v" / "attn" / "ln2" / "fc1"; "q" carries the head_dim^-0.5 scaling, which the
+        # engine applies after its rounding), every encoder LayerNorm input ("layers.{i}.ln1_in" / "ln2_in", "ln_f_in")
+        # and the attention scores ("layers.{i}.scores", [H, S, S], scaled)
+        self.enc_probe = None
 
     def __getitem__(self, k: str) -> torch.Tensor:
         return self.sd[k]
@@ -167,17 +173,21 @@ def _merge_heads(x: torch.Tensor) -> torch.Tensor:
 # --------------------------------------------------------------------------------------
 # a2. encoder
 # --------------------------------------------------------------------------------------
-def _flash_attention_engine_rounding(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, block: int = 64) -> torch.Tensor:
+def _flash_attention_engine_rounding(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, block: int = 64,
+                                     probe=None) -> torch.Tensor:
     """softmax(q k^T) v with the engine's rounding points: the same mathematics as the plain
     softmax, evaluated in 64-key blocks with a running row maximum, the un-normalised
     probabilities rounded to fp16 before they multiply V (they are the fp16 operand of the P*V
-    tensor-core MMA in ``enc_attn.cu``), the row sum kept in fp32.  ``q`` already carries the
-    head_dim^-0.5 scaling."""
+    tensor-core MMA in ``enc_attn.cu``), the row sum kept unrounded, in the working dtype.  ``q`` already carries the
+    head_dim^-0.5 scaling; ``probe`` (optional) sees the scores."""
     H, S, dh = q.shape
     s = q @ k.transpose(1, 2)
-    m = torch.full((H, S), float("-inf"))
-    l = torch.zeros(H, S)
-    o = torch.zeros(H, S, dh)
+    if probe is not None:
+        probe(s)
+    like = dict(dtype=q.dtype, device=q.device)
+    m = torch.full((H, S), float("-inf"), **like)
+    l = torch.zeros(H, S, **like)
+    o = torch.zeros(H, S, dh, **like)
     for b in range(0, S, block):
         sb = s[:, :, b : b + block]
         m_new = torch.maximum(m, sb.max(dim=-1).values)
@@ -196,13 +206,28 @@ def encoder_forward(w: RefWeights, cfg, mel: torch.Tensor, regime: str = "fp32")
     Follows HF ``modeling_whisper.py:593-647`` (``WhisperEncoder.forward``): conv1+GELU,
     conv2(stride 2)+GELU, + sinusoid positions, N pre-LN layers (``:380-414``; attention
     ``:284-357`` with q scaled before QK^T and no k bias), final LayerNorm.
+
+    Computes in ``w.dtype``.  In the engine regime the engine's fp16 rounding points are kept (the mel;
+    conv1 + GELU; the LayerNorm outputs; Q, K and V; P; the attention output; the FC1 + GELU output) and everything else
+    is in the working dtype.  ``w.enc_probe`` (optional) sees each of them before it is rounded.
     """
     eng = regime == "engine"
-    rq = _r16 if eng else (lambda t: t)
+    probe = w.enc_probe
+
+    def rq(name: str, t: torch.Tensor) -> torch.Tensor:
+        if probe is not None:
+            probe(name, t)
+        return _r16(t) if eng else t
+
+    def ln(name: str, t: torch.Tensor, prefix: str) -> torch.Tensor:
+        if probe is not None:
+            probe(name + "_in", t)
+        return w.ln(t, prefix)
+
     p = "whisper_model.model.encoder"
-    x = rq(mel.to(torch.float32))[None]  # [1, 80, 3000]
+    x = rq("mel", mel.to(w.dtype))[None]  # [1, 80, 3000]
     x = F.gelu(F.conv1d(x, w[f"{p}.conv1.weight"], w[f"{p}.conv1.bias"], padding=1))
-    x = rq(x)
+    x = rq("conv1", x)
     x = F.gelu(F.conv1d(x, w[f"{p}.conv2.weight"], w[f"{p}.conv2.bias"], stride=2, padding=1))
     x = x[0].transpose(0, 1)  # [1500, d]
     x = x + w[f"{p}.embed_positions.weight"]
@@ -210,21 +235,25 @@ def encoder_forward(w: RefWeights, cfg, mel: torch.Tensor, regime: str = "fp32")
     dh = cfg.d_model // H
     for i in range(cfg.encoder_layers):
         lp = f"{p}.layers.{i}"
-        h = rq(w.ln(x, f"{lp}.self_attn_layer_norm"))
+        li = f"layers.{i}."
+        h = rq(li + "ln1", ln(li + "ln1", x, f"{lp}.self_attn_layer_norm"))
         q = w.lin(h, f"{lp}.self_attn.q_proj") * (dh ** -0.5)
         k = w.lin(h, f"{lp}.self_attn.k_proj")
         v = w.lin(h, f"{lp}.self_attn.v_proj")
-        q, k, v = (_split_heads(rq(t), H) for t in (q, k, v))
+        q, k, v = (_split_heads(rq(li + n, t), H) for n, t in (("q", q), ("k", k), ("v", v)))
+        sprobe = (lambda s: probe(li + "scores", s)) if probe is not None else None
         if eng:
-            o = _merge_heads(_flash_attention_engine_rounding(q, k, v))
+            o = _merge_heads(_flash_attention_engine_rounding(q, k, v, probe=sprobe))
         else:
-            att = torch.softmax(q @ k.transpose(1, 2), dim=-1)
-            o = _merge_heads(att @ v)
-        x = x + w.lin(rq(o), f"{lp}.self_attn.out_proj")
-        h = rq(w.ln(x, f"{lp}.final_layer_norm"))
-        h = rq(F.gelu(w.lin(h, f"{lp}.fc1")))
+            s = q @ k.transpose(1, 2)
+            if sprobe is not None:
+                sprobe(s)
+            o = _merge_heads(torch.softmax(s, dim=-1) @ v)
+        x = x + w.lin(rq(li + "attn", o), f"{lp}.self_attn.out_proj")
+        h = rq(li + "ln2", ln(li + "ln2", x, f"{lp}.final_layer_norm"))
+        h = rq(li + "fc1", F.gelu(w.lin(h, f"{lp}.fc1")))
         x = x + w.lin(h, f"{lp}.fc2")
-    return w.ln(x, f"{p}.layer_norm")
+    return ln("ln_f", x, f"{p}.layer_norm")
 
 
 # --------------------------------------------------------------------------------------

@@ -37,15 +37,21 @@ def check_logits(engine, ref64, case, what, ref32=None, bar=None):
     In recording mode the error is written out instead of asserted."""
     engine = np.asarray(engine)
     assert np.isfinite(engine).all(), (case, what, "non-finite logits")
-    err = rel_err(engine, ref64)
+    return check_error(rel_err(engine, ref64), DECODE_LOGIT_BAR if bar is None else bar, case, what,
+                       None if ref32 is None else rel_err(ref32, ref64))
+
+
+def check_error(err, bar, case, what, oracle_fp32_err=None):
+    """Assert ``err <= bar``; in recording mode append the error (and the fp32 oracle's error against the same fp64
+    reference, if given) to the record file instead.  Returns ``err``."""
     if RECORD:
         rec = {"case": case, "what": what, "err": err}
-        if ref32 is not None:
-            rec["oracle_fp32_err"] = rel_err(ref32, ref64)
+        if oracle_fp32_err is not None:
+            rec["oracle_fp32_err"] = oracle_fp32_err
         with open(RECORD, "a") as f:
             f.write(json.dumps(rec) + "\n")
     else:
-        assert err <= (DECODE_LOGIT_BAR if bar is None else bar), (case, what, err)
+        assert err <= bar, (case, what, err, bar)
     return err
 
 

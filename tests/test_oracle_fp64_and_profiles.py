@@ -29,6 +29,7 @@ def test_default_state_dict_is_unchanged(preset, heads, htype, seed, digest):
     cfg = preset_config(preset, heads=heads, heads_type=htype)
     assert _digest(synthetic_state_dict(cfg, seed=seed)) == digest
     assert _digest(synthetic_state_dict(cfg, seed=seed, activation_profile="default")) == digest
+    assert _digest(synthetic_state_dict(cfg, seed=seed, encoder_profile="default")) == digest
 
 
 def test_width_config_and_d_model_override():

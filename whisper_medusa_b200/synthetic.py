@@ -45,11 +45,13 @@ def _decoder_layer_keys(prefix: str, d: int, ffn: int):
 
 
 ACTIVATION_PROFILES = ("default", "offset", "outliers", "gamma_spread", "small", "near_top")
+ENCODER_PROFILES = ("default", "offset", "outliers", "small", "peaked", "near_top")
 
 
 def synthetic_state_dict(config: MedusaConfig, seed: int = 0, enc_gain: float = 1.0,
                          dec_gain: float = 2.0, head_gain: float = 0.8,
-                         logit_std: float = 1.75, activation_profile: str = "default") -> Dict[str, torch.Tensor]:
+                         logit_std: float = 1.75, activation_profile: str = "default",
+                         encoder_profile: str = "default") -> Dict[str, torch.Tensor]:
     """Deterministic fp16 state dict of the exact shapes of ``config`` (CPU tensors).
 
     Linear weights are N(0, gain^2 / fan_in).  The gains are chosen (empirically, see
@@ -61,10 +63,13 @@ def synthetic_state_dict(config: MedusaConfig, seed: int = 0, enc_gain: float = 
 
     ``activation_profile`` (one of ``ACTIVATION_PROFILES``) reshapes the decoder side so that its residual stream and
     LayerNorm operands have the statistics of real checkpoints (see ``_apply_activation_profile``); ``"default"``
-    returns exactly the tensors it always did.
+    returns exactly the tensors it always did.  ``encoder_profile`` (one of ``ENCODER_PROFILES``) does the same for the
+    encoder's tensors (``_apply_encoder_profile``).
     """
     if activation_profile not in ACTIVATION_PROFILES:
         raise ValueError(f"activation_profile must be one of {ACTIVATION_PROFILES}")
+    if encoder_profile not in ENCODER_PROFILES:
+        raise ValueError(f"encoder_profile must be one of {ENCODER_PROFILES}")
     g = torch.Generator(device="cpu")
     g.manual_seed(int(seed))
     d, V = config.d_model, config.vocab_size
@@ -122,7 +127,107 @@ def synthetic_state_dict(config: MedusaConfig, seed: int = 0, enc_gain: float = 
             add(name, kind, shape)
     if activation_profile != "default":
         _apply_activation_profile(sd, config, activation_profile, seed)
+    if encoder_profile != "default":
+        _apply_encoder_profile(sd, config, encoder_profile, seed)
     return sd
+
+
+def _apply_encoder_profile(sd: Dict[str, torch.Tensor], config: MedusaConfig, profile: str, seed: int) -> None:
+    """Reshape the encoder tensors of ``sd`` in place (own generator: the default tensors are drawn first and
+    unchanged).  Nothing outside the encoder changes.
+
+    * ``offset``: a DC component common to all channels of the residual stream, through the conv2 bias (+20, which
+      GELU passes on), the position table (a per-row level cycling over 1, 10, 100, 300) and the O-proj / FC2 biases
+      (+5 each).  |mean| / std at the LayerNorm inputs reaches the hundreds; LayerNorm removes it exactly, so only the
+      fp32 residual stream and the LayerNorm statistics see it.
+    * ``outliers``: three residual channels 50-300x the others (position table, conv2 / O-proj / FC2 rows).
+    * ``small``: the residual stream scaled to std ~ 3e-3 (conv2 weights and bias, position table, O-proj / FC2), so the
+      LayerNorm eps of 1e-5 is a large share of the variance.
+    * ``peaked``: the Q and K rows of two heads per layer scaled by 3 (scores x 9): score spreads of tens, a near one-hot
+      softmax whose row maximum moves from one 64-key block to another.
+    * ``near_top``: in every layer one head's Q and V rows and a quarter of the FC1 neurons are scaled by 4000, so Q,
+      V and the FC1 + GELU output reach 1e4-3e4 at their fp16 rounding points; that head's K rows and the O-proj / FC2
+      columns that read the scaled values are scaled by 1/4000 (the scores and the function stay as they were).
+    """
+    g = torch.Generator(device="cpu")
+    g.manual_seed(2_000_003 * (ENCODER_PROFILES.index(profile) + 1) + int(seed))
+    d, f = config.d_model, config.encoder_ffn_dim
+    dh = d // config.encoder_attention_heads
+    enc = "whisper_model.model.encoder"
+    layers = [f"{enc}.layers.{i}" for i in range(config.encoder_layers)]
+    writers = ("self_attn.out_proj", "fc2")
+    pos = f"{enc}.embed_positions.weight"
+
+    def f32(k):
+        return sd[k].to(torch.float32)
+
+    def put(k, v):
+        v = v.to(torch.float16)
+        assert torch.isfinite(v).all(), k
+        sd[k] = v
+
+    if profile == "offset":
+        n_pos = sd[pos].shape[0]
+        dc = torch.tensor([1.0, 10.0, 100.0, 300.0]).repeat(n_pos // 4 + 1)[:n_pos]
+        put(pos, f32(pos) + dc[:, None])
+        put(f"{enc}.conv2.bias", f32(f"{enc}.conv2.bias") + 20.0)
+        for lp in layers:
+            for wr in writers:
+                put(f"{lp}.{wr}.bias", f32(f"{lp}.{wr}.bias") + 5.0)
+    elif profile == "outliers":
+        ch = torch.randperm(d, generator=g)[:3]
+        gain = torch.tensor([50.0, 120.0, 300.0])
+        p = f32(pos)
+        p[:, ch] = p[:, ch] * gain + 0.02 * gain
+        put(pos, p)
+        for k in ([f"{enc}.conv2"] + [f"{lp}.{wr}" for lp in layers for wr in writers]):
+            w, b = f32(f"{k}.weight"), f32(f"{k}.bias")
+            w[ch] *= gain.view(-1, *([1] * (w.dim() - 1)))
+            b[ch] *= gain
+            put(f"{k}.weight", w)
+            put(f"{k}.bias", b)
+    elif profile == "small":
+        s = 3e-3
+        for k in ([f"{enc}.conv2.weight", f"{enc}.conv2.bias", pos]
+                  + [f"{lp}.{wr}.{t}" for lp in layers for wr in writers for t in ("weight", "bias")]):
+            put(k, f32(k) * s)
+    elif profile == "peaked":
+        for lp in layers:
+            heads = torch.randperm(config.encoder_attention_heads, generator=g)[:2]
+            for proj in ("q_proj", "k_proj"):
+                w = f32(f"{lp}.self_attn.{proj}.weight")
+                b = f32(f"{lp}.self_attn.{proj}.bias") if proj == "q_proj" else None
+                for h in heads.tolist():
+                    w[h * dh:(h + 1) * dh] *= 3.0
+                    if b is not None:
+                        b[h * dh:(h + 1) * dh] *= 3.0
+                put(f"{lp}.self_attn.{proj}.weight", w)
+                if b is not None:
+                    put(f"{lp}.self_attn.{proj}.bias", b)
+    elif profile == "near_top":
+        G = 4000.0
+        for lp in layers:
+            h = int(torch.randint(config.encoder_attention_heads, (1,), generator=g))
+            rows = slice(h * dh, (h + 1) * dh)
+            for proj, scale in (("q_proj", G), ("k_proj", 1.0 / G), ("v_proj", G)):
+                w = f32(f"{lp}.self_attn.{proj}.weight")
+                w[rows] *= scale
+                put(f"{lp}.self_attn.{proj}.weight", w)
+                if proj != "k_proj":
+                    b = f32(f"{lp}.self_attn.{proj}.bias")
+                    b[rows] *= scale
+                    put(f"{lp}.self_attn.{proj}.bias", b)
+            wo = f32(f"{lp}.self_attn.out_proj.weight")
+            wo[:, rows] /= G
+            put(f"{lp}.self_attn.out_proj.weight", wo)
+            nrn = torch.randperm(f, generator=g)[: f // 4]
+            w1, b1, w2 = f32(f"{lp}.fc1.weight"), f32(f"{lp}.fc1.bias"), f32(f"{lp}.fc2.weight")
+            w1[nrn] *= G
+            b1[nrn] *= G
+            w2[:, nrn] /= G
+            put(f"{lp}.fc1.weight", w1)
+            put(f"{lp}.fc1.bias", b1)
+            put(f"{lp}.fc2.weight", w2)
 
 
 def _apply_activation_profile(sd: Dict[str, torch.Tensor], config: MedusaConfig, profile: str, seed: int) -> None:
