@@ -16,8 +16,6 @@
 
 namespace wm {
 
-struct StageInstr;
-
 // Candidate tree of a branching `medusa_choices` (reference medusa_utils.py:305-421 generate_medusa_buffers; built by the
 // host in wm_set_medusa_choices).  Nodes are numbered level by level; node 0 = the base-head token.  The engine holds at
 // most WM_MAX_T nodes, WM_TREE_MAX_CAND root-to-leaf paths and WM_TREE_MAX_TOPK candidates per head.
@@ -260,8 +258,7 @@ struct alignas(16) DecModel {   // (copied to shared memory in 16-byte pieces by
   int sel_nseg;       // vocabulary segments per row of the logits scan: clamp(n_sm / (K+1), 1, 32)
   float* logits_a;    // [WM_MAX_T, V]
   float* logits_b;    // [WM_MAX_T, V]
-  // stage program of the persistent ring kernel: {stage, mode, layer} triples; lists [off[i], off[i+1])
-  const struct StageInstr* prog;
+  // instruction lists of the ring kernel's stage program (dec_build_program): sweep A, tail, verify = [off[i], off[i+1])
   int prog_off[4];
   // per-CTA weight-chunk schedule of the ring producer (built by the host once the weights are bound):
   // chunk_tab[chunk_off[cta*4 + list] .. chunk_off[cta*4 + list + 1]) in consumption order
@@ -270,7 +267,7 @@ struct alignas(16) DecModel {   // (copied to shared memory in 16-byte pieces by
   const struct CtaStage* stage_tab;   // [prog_off[3]][n_sm] resolved stage records of the ring kernel
   DecState* st;
   unsigned int* bar;  // grid-barrier words for the persistent kernel
-  unsigned long long* prof;  // optional stage timeline [2 CTAs][n_instr][3] (ns), null = off
+  unsigned long long* prof;  // optional stage timeline [2 CTAs][n_instr][16] (ns, and flags), null = off
 };
 
 }  // namespace wm

@@ -38,20 +38,23 @@ struct PassGeom {
   int T;     // query rows of this pass
   int base;  // position of row 0 (also the self-KV row it writes)
 };
-__device__ __forceinline__ PassGeom pass_geom(const DecModel* m, int mode) {
-  const DecState* st = m->st;
+// L, kv_len: the loop state's; n_tree: rows of the verify pass
+__host__ __device__ __forceinline__ PassGeom pass_geom(int mode, int L, int kv_len, int n_tree) {
   PassGeom g;
   if (mode == MODE_A) {
-    g.T = st->L - st->kv_len;
-    g.base = st->kv_len;
+    g.T = L - kv_len;
+    g.base = kv_len;
   } else if (mode == MODE_B) {
-    g.T = m->n_tree;
-    g.base = st->L;
+    g.T = n_tree;
+    g.base = L;
   } else {
     g.T = 1;
-    g.base = st->L - 1;
+    g.base = L - 1;
   }
   return g;
+}
+__device__ __forceinline__ PassGeom pass_geom(const DecModel* m, int mode) {
+  return pass_geom(mode, m->st->L, m->st->kv_len, m->n_tree);
 }
 
 // -----------------------------------------------------------------------------------------
@@ -468,6 +471,19 @@ __host__ __device__ constexpr size_t cross_attn_smem_bytes() {
   return (size_t)2 * WM_CH_PAD * 72 * sizeof(__half) + (size_t)WM_MAX_T * WM_SS_STRIDE * sizeof(float) +
          (size_t)2 * 16 * 72 * sizeof(__half) + (size_t)2 * WM_MAX_T * sizeof(float);   // K, V chunk + cross_scratch_bytes()
 }
+// Item `item` of the stage = key chunk c of head h: encoder positions [j0, j0 + nk) of S (nk = 0: an empty trailing
+// chunk).
+// The stage kernels, the ring kernel and the ring's chunk schedule all take their items from here.
+struct CrossItem { int h, c, j0, nk; };
+__host__ __device__ __forceinline__ CrossItem cross_item(int item, int S, int nch) {
+  const int CH = (S + nch - 1) / nch;
+  CrossItem it;
+  it.h = item / nch;
+  it.c = item - it.h * nch;
+  it.j0 = it.c * CH;
+  it.nk = max(0, min(S, it.j0 + CH) - it.j0);
+  return it;
+}
 __device__ __forceinline__ void split_hilo(float a, float b, uint32_t& hi, uint32_t& lo) {
   const __half ha = __float2half_rn(a), hb = __float2half_rn(b);
   __half2 h = __halves2half2(ha, hb);
@@ -668,14 +684,13 @@ __device__ __forceinline__ void stage_cross_attn(const DecModel* m, int mode, in
   const int H = m->H, S = m->S;
   const DecLayer& L = m->layers[layer];
   const int nch = m->cross_chunks;
-  const int CH = (S + nch - 1) / nch;
   __half* sK = reinterpret_cast<__half*>(smem_raw);                 // [CH_PAD][72]
   __half* sV = sK + WM_CH_PAD * 72;                                 // [CH_PAD][72]
   const CrossScratch cs = cross_scratch(reinterpret_cast<unsigned char*>(sV + WM_CH_PAD * 72));
   const int tid = threadIdx.x;
   for (int item = cta; item < H * nch; item += ncta) {
-    const int h = item / nch, c = item - h * nch;
-    const int j0 = c * CH, nk = max(0, min(S, j0 + CH) - j0);
+    const CrossItem it = cross_item(item, S, nch);
+    const int h = it.h, c = it.c, j0 = it.j0, nk = it.nk;
     const int nk_pad = (nk + 15) & ~15;
     cta_sync();
     // K / V chunk -> shared memory (all loads of a batch in flight before the first store); the cache rows are
@@ -1242,7 +1257,7 @@ enum StageId {
 enum PhaseId { PH_SWEEP_A = 0, PH_TAIL = 1, PH_VERIFY = 2 };
 
 // (host: called with the host copy of the model and an explicit geometry -- x_rows / base of the pass
-// are placeholders there, see dec_build_stage_table)
+// are placeholders there, see dec_build_ring_tables)
 __host__ __device__ GemmDesc make_gemm_desc(const DecModel* m, int stage, int mode, int layer, const PassGeom* gopt) {
 #ifdef __CUDA_ARCH__
   const PassGeom pg = gopt ? *gopt : pass_geom(m, mode);
@@ -1478,55 +1493,6 @@ size_t dec_ring_smem_bytes(int d) {
   }
 }
 
-// Per-CTA chunk schedule of the ring producer, in exactly the order stage_gemm_ring consumes:
-// for every GEMM stage of the program with work for the CTA (gemm_work): for unit (16 rows).
-// `hm` is the HOST copy of the model (device pointers inside).  off has 4 entries per CTA.
-void dec_build_chunk_table(const DecModel& hm, int ncta, std::vector<ChunkDesc>& tab, std::vector<int>& off) {
-  std::vector<int> flat;
-  int poff[4];
-  dec_build_program(hm.n_layers, hm.has_block, flat, poff);
-  tab.clear();
-  off.assign((size_t)ncta * 4, 0);
-  for (int cta = 0; cta < ncta; ++cta) {
-    for (int list = 0; list < 3; ++list) {
-      off[(size_t)cta * 4 + list] = (int)tab.size();
-      for (int ip = poff[list]; ip < poff[list + 1]; ++ip) {
-        const int stage = flat[ip * 3], mode = flat[ip * 3 + 1], layer = flat[ip * 3 + 2];
-        if (stage == ST_CROSS_ATTN) {
-          // the K and the V rows of every (head, key chunk) item of this CTA: one contiguous copy each
-          const int nch = hm.cross_chunks, CH = (hm.S + nch - 1) / nch;
-          for (int item = cta; item < hm.H * nch; item += ncta) {
-            const int hh = item / nch, cc = item - hh * nch;
-            const int j0 = cc * CH, nk = std::max(0, std::min(hm.S, j0 + CH) - j0);
-            if (nk == 0) continue;
-            ChunkDesc c;
-            c.row_bytes = 0; c.nrows = 1; c.copy_bytes = (uint32_t)(nk * 72 * sizeof(__half));
-            c.src = hm.layers[layer].cross_k + ((size_t)hh * hm.S_pad + j0) * 72;
-            tab.push_back(c);
-            c.src = hm.layers[layer].cross_v + ((size_t)hh * hm.S_pad + j0) * 72;
-            tab.push_back(c);
-          }
-          continue;
-        }
-        if (!is_gemm_stage(stage)) continue;
-        const WDesc w = stage_weights(&hm, stage, mode, layer);
-        const GemmWork wk = gemm_work(w.N, w.K, hm.d, cta, ncta);
-        if (wk.n_rows == 0) continue;
-        const int units = (wk.n_rows + 15) >> 4;
-        for (int u = 0; u < units; ++u) {
-          ChunkDesc c;
-          c.src = w.W + (size_t)(wk.n_begin + u * 16) * w.K + (size_t)wk.seg * hm.d;
-          c.row_bytes = (uint32_t)(w.K * sizeof(__half));
-          c.nrows = (uint32_t)std::min(16, wk.n_rows - u * 16);
-          c.copy_bytes = (uint32_t)(hm.d * sizeof(__half));
-          tab.push_back(c);
-        }
-      }
-    }
-    off[(size_t)cta * 4 + 3] = (int)tab.size();
-  }
-}
-
 // Derived vectors of the LayerNorm-fed GEMMs (QKV, cross-Q, FC1) of the ring kernel, {b'_n, c_n} with
 //     c_n = sum_k gamma_k W_nk,   b'_n = b_n + sum_k beta_k W_nk
 // so that LN(x) W^T + b = rstd * ((gamma o x) W^T - mu * c) + b' (stage_gemm_ring).  Layout per decoder layer (the Medusa
@@ -1570,91 +1536,127 @@ cudaError_t dec_fold_layernorms(const DecModel& hm, int n_dec, float2* out, cuda
   return cudaGetLastError();
 }
 
-// Resolved stage records of the ring kernel: tab[ip * ncta + cta] (see CtaStage in common.cuh).  `cluster`: CTAs per
-// cluster of the launch the table is for (dec_ring_cluster_size).
-void dec_build_stage_table(const DecModel& hm, const float2* ln_fold, int ncta, int cluster, std::vector<CtaStage>& tab) {
+// The host tables of the ring kernel, built in one walk of the stage program, so that the chunks the producer warp
+// streams into the ring and the slots the compute warps take back out come from the same record.  `hm` is the HOST copy
+// of the model (device pointers inside); `cluster`: CTAs per cluster of the launch the tables are for
+// (dec_ring_cluster_size).
+//   stab[ip * ncta + cta]: the resolved record of instruction ip for CTA cta (CtaStage in common.cuh);
+//   ctab[off[cta * 4 + list] .. off[cta * 4 + list + 1]): the chunks of CTA cta for program list `list`, in the order
+//   they are consumed: one per 16 rows of a GEMM record (stage_gemm_ring), the K and the V rows of every
+//   cross-attention item of the CTA (stage_cross_attn_ring).
+void dec_build_ring_tables(const DecModel& hm, const float2* ln_fold, int ncta, int cluster, std::vector<CtaStage>& stab,
+                           std::vector<ChunkDesc>& ctab, std::vector<int>& off) {
   std::vector<int> flat;
   int poff[4];
   dec_build_program(hm.n_layers, hm.has_block, flat, poff);
   const int n = poff[3];
-  tab.assign((size_t)n * ncta, CtaStage{});
   const PassGeom dyn{-1, 0};   // T = -1: "the rows of the pass" (resolved on the device)
+  auto desc = [&](int ip) { return make_gemm_desc(&hm, flat[ip * 3], flat[ip * 3 + 1], flat[ip * 3 + 2], &dyn); };
   // bias the ring kernel reads for a GEMM stage: LayerNorm stages read the {b'_n, c_n} pairs (8 bytes per row)
-  auto ring_bias = [&](const GemmDesc& g, int stage, int layer, size_t& row_bytes) -> const float* {
+  auto ring_bias = [&](const GemmDesc& g, int ip, size_t& row_bytes) -> const float* {
     if (g.xsrc == XS_LN) {
       row_bytes = sizeof(float2);
-      return reinterpret_cast<const float*>(ln_fold + ln_fold_offset(stage, layer, hm.d, hm.ffn));
+      return reinterpret_cast<const float*>(ln_fold + ln_fold_offset(flat[ip * 3], flat[ip * 3 + 2], hm.d, hm.ffn));
     }
     row_bytes = sizeof(float);
     return g.bias;
   };
-  for (int ip = 0; ip < n; ++ip) {
-    const int stage = flat[ip * 3], mode = flat[ip * 3 + 1], layer = flat[ip * 3 + 2];
-    // LayerNorm gamma of the next instruction (bulk-copied into shared memory while this one runs) ...
-    const float* nx_g = nullptr;
-    if (ip + 1 < n && is_gemm_stage(flat[(ip + 1) * 3])) {
-      const GemmDesc gn = make_gemm_desc(&hm, flat[(ip + 1) * 3], flat[(ip + 1) * 3 + 1], flat[(ip + 1) * 3 + 2], &dyn);
-      if (gn.xsrc == XS_LN) nx_g = gn.ln_g;
+  auto push_chunk = [&](const void* src, size_t row_bytes, int nrows, size_t copy_bytes) {
+    ctab.push_back(ChunkDesc{src, (uint32_t)row_bytes, (uint32_t)nrows, (uint32_t)copy_bytes, 0u});
+  };
+  // LayerNorm gamma of the next instruction (bulk-copied into shared memory while this one runs)
+  std::vector<const float*> nx_g(n, nullptr);
+  for (int ip = 0; ip + 1 < n; ++ip)
+    if (is_gemm_stage(flat[(ip + 1) * 3])) {
+      const GemmDesc gn = desc(ip + 1);
+      if (gn.xsrc == XS_LN) nx_g[ip] = gn.ln_g;
     }
-    // ... and the next GEMM stage (bias prefetch)
-    int jn = -1;
-    for (int jp = ip + 1; jp < n && jp < ip + 4; ++jp)
-      if (is_gemm_stage(flat[jp * 3])) { jn = jp; break; }
-    for (int cta = 0; cta < ncta; ++cta) {
-      CtaStage& c = tab[(size_t)ip * ncta + cta];
-      c.stage = stage; c.mode = mode; c.layer = layer;
-      c.nx_g = nx_g;
-      if (jn >= 0) {
-        const GemmDesc gn = make_gemm_desc(&hm, flat[jn * 3], flat[jn * 3 + 1], flat[jn * 3 + 2], &dyn);
-        const GemmWork wn = gemm_work(gn.N, gn.K, hm.d, cta, ncta);
-        size_t rb = 0;
-        const float* nb = ring_bias(gn, flat[jn * 3], flat[jn * 3 + 2], rb);
-        if (nb && wn.n_rows > 0) {
-          const uintptr_t a0 = ((uintptr_t)nb + wn.n_begin * rb) & ~(uintptr_t)127;
-          const uintptr_t a1 = (uintptr_t)nb + (wn.n_begin + wn.n_rows) * rb;
-          c.pf_bias = reinterpret_cast<const float*>(a0);
-          c.pf_bias_lines = (int)std::min<uintptr_t>(32, (a1 - a0 + 127) / 128);
+  stab.assign((size_t)n * ncta, CtaStage{});
+  ctab.clear();
+  off.assign((size_t)ncta * 4, 0);
+  for (int cta = 0; cta < ncta; ++cta) {
+    for (int list = 0; list < 3; ++list) {
+      off[(size_t)cta * 4 + list] = (int)ctab.size();
+      for (int ip = poff[list]; ip < poff[list + 1]; ++ip) {
+        const int stage = flat[ip * 3], layer = flat[ip * 3 + 2];
+        CtaStage& c = stab[(size_t)ip * ncta + cta];
+        c.stage = stage; c.mode = flat[ip * 3 + 1]; c.layer = layer;
+        c.nx_g = nx_g[ip];
+        // this CTA's bias slice of the next GEMM stage, if one follows within three instructions (L2 prefetch)
+        for (int jn = ip + 1; jn < n && jn < ip + 4; ++jn) {
+          if (!is_gemm_stage(flat[jn * 3])) continue;
+          const GemmDesc gn = desc(jn);
+          const GemmWork wn = gemm_work(gn.N, gn.K, hm.d, cta, ncta);
+          size_t rb = 0;
+          const float* nb = ring_bias(gn, jn, rb);
+          if (nb && wn.n_rows > 0) {
+            const uintptr_t a0 = ((uintptr_t)nb + wn.n_begin * rb) & ~(uintptr_t)127;
+            const uintptr_t a1 = (uintptr_t)nb + (wn.n_begin + wn.n_rows) * rb;
+            c.pf_bias = reinterpret_cast<const float*>(a0);
+            c.pf_bias_lines = (int)std::min<uintptr_t>(32, (a1 - a0 + 127) / 128);
+          }
+          break;
         }
-      }
-      if (!is_gemm_stage(stage)) continue;
-      const GemmDesc g = make_gemm_desc(&hm, stage, mode, layer, &dyn);
-      const GemmWork wk = gemm_work(g.N, g.K, hm.d, cta, ncta);
-      c.epi = g.epi;
-      c.ln = (g.xsrc == XS_LN) ? 1 : 0;
-      c.X = g.X + (size_t)g.x_row0 * g.K + (size_t)wk.seg * hm.d;
-      c.x_ld = g.K;
-      c.x_rows_fixed = g.x_rows < 0 ? 0 : g.x_rows;
-      size_t rb = 0;
-      c.bias = ring_bias(g, stage, layer, rb);
-      c.out = g.out;
-      c.n_begin = wk.n_begin; c.n_rows = wk.n_rows;
-      c.N = g.N; c.ldo = g.ldo; c.out_row0 = g.out_row0;
-      c.segs = wk.segs; c.seg = wk.seg; c.block = wk.block;
-      // activations that only ever feed one GEMM stage travel in the MMA operand format: the attention stages and
-      // the GELU epilogue of FC1 write it, O-proj / cross-O / FC2 skip their split pass.  The residual stream feeds a
-      // LayerNorm GEMM: the residual epilogue before one also writes gamma o x in that format (xg), and that stage
-      // stages xg instead of x (layer 0 and the Medusa block, fed by other stages, split gamma o x themselves)
-      const bool resid = (stage == ST_OPROJ || stage == ST_CROSS_O || stage == ST_FC2);
-      c.presplit = resid ? 1 : 0;
-      c.out_split = (stage == ST_FC1) ? 1 : 0;
-      if (resid && nx_g) c.out_gx = hm.xg;
-      if (c.ln && ip > 0) {
-        const int ps = flat[(ip - 1) * 3];
-        if (ps == ST_OPROJ || ps == ST_CROSS_O || ps == ST_FC2) { c.presplit = 1; c.X = hm.xg; }
+        if (stage == ST_CROSS_ATTN) {
+          // the K and the V rows of every (head, key chunk) item of this CTA: one contiguous copy each
+          const DecLayer& L = hm.layers[layer];
+          for (int item = cta; item < hm.H * hm.cross_chunks; item += ncta) {
+            const CrossItem it = cross_item(item, hm.S, hm.cross_chunks);
+            if (it.nk == 0) continue;
+            const size_t row0 = ((size_t)it.h * hm.S_pad + it.j0) * 72;
+            push_chunk(L.cross_k + row0, 0, 1, it.nk * 72 * sizeof(__half));
+            push_chunk(L.cross_v + row0, 0, 1, it.nk * 72 * sizeof(__half));
+          }
+          continue;
+        }
+        if (!is_gemm_stage(stage)) continue;
+        const GemmDesc g = desc(ip);
+        const GemmWork wk = gemm_work(g.N, g.K, hm.d, cta, ncta);
+        c.epi = g.epi;
+        c.ln = (g.xsrc == XS_LN) ? 1 : 0;
+        c.X = g.X + (size_t)g.x_row0 * g.K + (size_t)wk.seg * hm.d;
+        c.x_ld = g.K;
+        c.x_rows_fixed = g.x_rows < 0 ? 0 : g.x_rows;
+        size_t rb = 0;
+        c.bias = ring_bias(g, ip, rb);
+        c.out = g.out;
+        c.n_begin = wk.n_begin; c.n_rows = wk.n_rows;
+        c.N = g.N; c.ldo = g.ldo; c.out_row0 = g.out_row0;
+        c.segs = wk.segs; c.seg = wk.seg; c.block = wk.block;
+        // activations that only ever feed one GEMM stage travel in the MMA operand format: the attention stages and
+        // the GELU epilogue of FC1 write it, O-proj / cross-O / FC2 skip their split pass.  The residual stream feeds a
+        // LayerNorm GEMM: the residual epilogue before one also writes gamma o x in that format (xg), and that stage
+        // stages xg instead of x (layer 0 and the Medusa block, fed by other stages, split gamma o x themselves)
+        const bool resid = (stage == ST_OPROJ || stage == ST_CROSS_O || stage == ST_FC2);
+        c.presplit = resid ? 1 : 0;
+        c.out_split = (stage == ST_FC1) ? 1 : 0;
+        if (resid && c.nx_g) c.out_gx = hm.xg;
+        if (c.ln && ip > 0) {
+          const int ps = flat[(ip - 1) * 3];
+          if (ps == ST_OPROJ || ps == ST_CROSS_O || ps == ST_FC2) { c.presplit = 1; c.X = hm.xg; }
+        }
+        // the weight rows of the record, 16 per chunk: d columns of k segment `seg`
+        for (int r = 0; r < c.n_rows; r += 16)
+          push_chunk(g.W + (size_t)(c.n_begin + r) * g.K + (size_t)c.seg * hm.d, g.K * sizeof(__half),
+                     std::min(16, c.n_rows - r), hm.d * sizeof(__half));
       }
     }
-    // 2-CTA clusters (CTAs 2i, 2i + 1): one multicast copy of X for both where they stage the same rows.  Both must have
-    // rows: a CTA without rows returns before staging, and the peer's complete_tx would then shift its xbar phase.
-    if (cluster == 2 && is_gemm_stage(stage))
+    off[(size_t)cta * 4 + 3] = (int)ctab.size();
+  }
+  // 2-CTA clusters (CTAs 2i, 2i + 1): one multicast copy of X for both where they stage the same rows.  Both must have
+  // rows: a CTA without rows returns before staging, and the peer's complete_tx would then shift its xbar phase.
+  if (cluster == 2)
+    for (int ip = 0; ip < n; ++ip) {
+      if (!is_gemm_stage(flat[ip * 3])) continue;
       for (int cta = 0; cta + 1 < ncta; cta += 2) {
-        CtaStage& a = tab[(size_t)ip * ncta + cta];
-        CtaStage& b = tab[(size_t)ip * ncta + cta + 1];
+        CtaStage& a = stab[(size_t)ip * ncta + cta];
+        CtaStage& b = stab[(size_t)ip * ncta + cta + 1];
         if (a.n_rows > 0 && b.n_rows > 0 && a.X == b.X && a.x_ld == b.x_ld && a.x_rows_fixed == b.x_rows_fixed) {
           a.x_role = XR_ISSUE;
           b.x_role = XR_RECEIVE;
         }
       }
-  }
+    }
 }
 
 cudaError_t dec_relayout_cross_kv(const __half* kv, __half* ck, __half* cv, int S, int S_pad, int d, int H, cudaStream_t s,
@@ -1767,7 +1769,7 @@ static int stage_grid(int stage, int T, int n_sm, int H, int K) {
 //   PH_VERIFY : sweep B + acceptance
 cudaError_t dec_enqueue_phase(const DecModel* dm, const DecHostInfo& hi, int phase, int T, cudaStream_t s, int64_t* n_launch) {
   auto launch = [&](int stage, int mode, int layer) {
-    const int rows = (mode == MODE_B) ? hi.n_tree : (mode == MODE_TAIL ? 1 : T);
+    const int rows = pass_geom(mode, T, 0, hi.n_tree).T;   // (sweep A over T rows: L = T, kv_len = 0)
     const int grid = stage_grid(stage, rows, hi.n_sm, hi.H, hi.K);
     dec_stage_kernel<<<grid, WM_DEC_THREADS, hi.smem, s>>>(dm, stage, mode, layer, phase);
     if (n_launch) ++*n_launch;

@@ -45,8 +45,6 @@
 #define WM_RING_G 3
 #define WM_RING_THREADS (WM_DEC_THREADS + 32)
 
-struct StageInstr { int stage, mode, layer; };
-
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
   asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
@@ -104,28 +102,6 @@ __device__ __forceinline__ void prefetch_l2(const void* p) { asm volatile("prefe
 __host__ __device__ __forceinline__ bool is_gemm_stage(int st) {
   return st == ST_QKV || st == ST_OPROJ || st == ST_CROSS_Q || st == ST_CROSS_O || st == ST_FC1 || st == ST_FC2 ||
          st == ST_HEADS || st == ST_VOCAB;
-}
-
-// static part of a GEMM stage (what the producer needs): weights and shape
-struct WDesc { const __half* W; int N, K; };
-__host__ __device__ inline WDesc stage_weights(const DecModel* m, int stage, int mode, int layer) {
-  const DecLayer& L = m->layers[layer];
-  const int d = m->d;
-  WDesc w;
-  switch (stage) {
-    case ST_QKV: w.W = L.qkv_w; w.N = 3 * d; w.K = d; break;
-    case ST_OPROJ: w.W = L.o_w; w.N = d; w.K = d; break;
-    case ST_CROSS_Q: w.W = L.cq_w; w.N = d; w.K = d; break;
-    case ST_CROSS_O: w.W = L.co_w; w.N = d; w.K = d; break;
-    case ST_FC1: w.W = L.fc1_w; w.N = m->ffn; w.K = d; break;
-    case ST_FC2: w.W = L.fc2_w; w.N = d; w.K = m->ffn; break;
-    case ST_HEADS:
-      w.W = m->heads_w; w.K = d;
-      w.N = (mode == MODE_A) ? (m->has_block ? m->K : m->K + 1) * d : d;
-      break;
-    default: w.W = m->embed; w.N = m->V; w.K = d; break;
-  }
-  return w;
 }
 
 __host__ __device__ __forceinline__ void cta_rows(int N, int part, int nparts, int& n_begin, int& n_rows) {
@@ -603,11 +579,10 @@ __device__ __forceinline__ void stage_cross_attn_ring(RingState& rs, unsigned ch
   uint64_t* const empty = full + WM_RING_G;
   const CrossScratch cs = cross_scratch(smem + G::SCRATCH_OFF);
   const int H = m->H, S = m->S, nch = m->cross_chunks;
-  const int CH = (S + nch - 1) / nch;
   const int tid = threadIdx.x;
   for (int item = cta; item < H * nch; item += ncta) {
-    const int h = item / nch, c = item - h * nch;
-    const int j0 = c * CH, nk = max(0, min(S, j0 + CH) - j0);
+    const CrossItem it = cross_item(item, S, nch);
+    const int h = it.h, c = it.c, nk = it.nk;
     if (nk == 0) continue;   // (no chunks in the table either)
     const int nk_pad = (nk + 15) & ~15;
     const int slot_k = rs.slot;
@@ -701,11 +676,8 @@ dec_iteration_ring_kernel(const DecModel* __restrict__ gm) {
     unsigned long long* pr = prof ? m->prof + ((size_t)(cta == 0 ? 0 : 1) * ip_last + ip) * 16 : nullptr;
     if (prof) pr[0] = global_timer_ns();
     const int stage = sd->stage, mode = sd->mode;
-    // the pass geometry derives from (L0, kv0, K): the loop state only changes in the very last stage
-    PassGeom pgv;
-    if (mode == MODE_A) { pgv.T = L0 - kv0; pgv.base = kv0; }
-    else if (mode == MODE_B) { pgv.T = m->n_tree; pgv.base = L0; }
-    else { pgv.T = 1; pgv.base = L0 - 1; }
+    // the pass geometry derives from (L0, kv0): the loop state only changes in the very last stage
+    const PassGeom pgv = pass_geom(mode, L0, kv0, m->n_tree);
     // LayerNorm gamma of the next stage -> its region (last read by an earlier LayerNorm stage; a LayerNorm stage never
     // precedes another), in flight while this stage runs: its residual epilogue (if any) reads it too
     if (threadIdx.x == 0 && sd->nx_g != nullptr) {

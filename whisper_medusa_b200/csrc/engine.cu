@@ -62,7 +62,7 @@ struct wm_handle {
   uint8_t* tok_mask = nullptr;
   float* pen_tab = nullptr;
   unsigned int* bar = nullptr;
-  int* prog = nullptr;
+  std::vector<int> prog;   // the ring kernel's stage program, {stage, mode, layer} per instruction (labels the profile)
   unsigned long long* prof = nullptr;
   ChunkDesc* chunk_tab = nullptr;
   int* chunk_off = nullptr;
@@ -346,13 +346,7 @@ extern "C" int wm_create(const wm_config* cfg, int device, wm_handle** out) {
   // product path by default: one persistent ring-kernel launch per speculative iteration.  Decoder widths the ring
   // kernel is not instantiated for (WM_RING_WIDTHS) fall back to the stage-kernel graphs.
   h->decode_mode = h->hi.smem_ring ? 2 : 0;
-  {
-    std::vector<int> flat;
-    dec_build_program(c.dec_layers, m.has_block, flat, m.prog_off);
-    CK(dalloc(&h->prog, flat.size()));
-    CK(cudaMemcpy(h->prog, flat.data(), flat.size() * sizeof(int), cudaMemcpyHostToDevice));
-    m.prog = reinterpret_cast<const StageInstr*>(h->prog);
-  }
+  dec_build_program(c.dec_layers, m.has_block, h->prog, m.prog_off);
   CK(enc_gemm_configure());
   h->tc_ok = (enc_gemm_tc_configure() == cudaSuccess);
   h->enc_gemm_impl = h->tc_ok ? 1 : 0;   // wgmma/TMA GEMM by default; option "enc_gemm" = 0 selects the mma.sync kernel
@@ -363,14 +357,20 @@ extern "C" int wm_create(const wm_config* cfg, int device, wm_handle** out) {
   return WM_OK;
 }
 
+// the cached graph-mode decode graphs: they bake in the grid and the verify rows
+static void drop_graphs(wm_handle* h) {
+  for (auto& kv : h->graph_a) cudaGraphExecDestroy(kv.second);
+  h->graph_a.clear();
+  if (h->graph_b) { cudaGraphExecDestroy(h->graph_b); h->graph_b = nullptr; }
+  if (h->graph_tail) { cudaGraphExecDestroy(h->graph_tail); h->graph_tail = nullptr; }
+}
+
 extern "C" int wm_destroy(wm_handle* h) {
   if (!h) return WM_OK;
   if (h->device < 0) { delete h; return WM_OK; }
   cudaSetDevice(h->device);
   if (h->stream) cudaStreamSynchronize(h->stream);
-  for (auto& kv : h->graph_a) cudaGraphExecDestroy(kv.second);
-  if (h->graph_b) cudaGraphExecDestroy(h->graph_b);
-  if (h->graph_tail) cudaGraphExecDestroy(h->graph_tail);
+  drop_graphs(h);
   auto F = [](void* p) { if (p) cudaFree(p); };
   F(h->pcm); F(h->mel32); F(h->melfb); F(h->gmax); F(h->x_tm); F(h->h1); F(h->x32); F(h->enc32); F(h->ln16);
   F(h->qkv16); F(h->att16); F(h->ffn16); F(h->enc16); F(h->vt16);
@@ -379,7 +379,7 @@ extern "C" int wm_destroy(wm_handle* h) {
   for (auto p : h->self_k) F(p);
   for (auto p : h->self_v) F(p);
   F(h->hm.x); F(h->hm.xg); F(h->hm.q); F(h->hm.attn); F(h->hm.ffn_h); F(h->hm.hidden); F(h->hm.head_h); F(h->hm.carry); F(h->hm.cross_part); F(h->hm.cross_cnt); F(h->hm.sel_part); F(h->hm.gemm_part); F(h->hm.gemm_cnt);
-  F(h->hm.topk_part); F(h->tree); F(h->hm.logits_a); F(h->hm.logits_b); F(h->st); F(h->tok_mask); F(h->pen_tab); F(h->bar); F(h->prog); F(h->prof); F(h->chunk_tab); F(h->chunk_off); F(h->stage_tab); F(h->ln_fold); F(h->dm);
+  F(h->hm.topk_part); F(h->tree); F(h->hm.logits_a); F(h->hm.logits_b); F(h->st); F(h->tok_mask); F(h->pen_tab); F(h->bar); F(h->prof); F(h->chunk_tab); F(h->chunk_off); F(h->stage_tab); F(h->ln_fold); F(h->dm);
   if (h->wowned) F(h->wdev);
   for (auto& kv : h->resamplers) { F(kv.second.taps); F(kv.second.sup); }
   if (h->h_state) cudaFreeHost(h->h_state);
@@ -451,23 +451,22 @@ static int bind_weights(wm_handle* h) {
   CK(dec_fold_layernorms(m, h->n_dec, h->ln_fold, h->stream));
   CK(cudaStreamSynchronize(h->stream));
   {
-    // weight-chunk schedule of the ring producer (depends on the weight addresses)
+    // stage records and weight-chunk schedule of the ring kernel (depend on the weight addresses and the grid)
+    std::vector<CtaStage> stab;
     std::vector<ChunkDesc> tab;
     std::vector<int> off;
-    dec_build_chunk_table(m, h->n_cta, tab, off);
+    dec_build_ring_tables(m, h->ln_fold, h->n_cta, h->hi.cluster, stab, tab, off);
     if (h->chunk_tab) { cudaFree(h->chunk_tab); h->chunk_tab = nullptr; }
     if (h->chunk_off) { cudaFree(h->chunk_off); h->chunk_off = nullptr; }
+    if (h->stage_tab) { cudaFree(h->stage_tab); h->stage_tab = nullptr; }
     CK(cudaMalloc((void**)&h->chunk_tab, tab.size() * sizeof(ChunkDesc)));
     CK(cudaMalloc((void**)&h->chunk_off, off.size() * sizeof(int)));
+    CK(cudaMalloc((void**)&h->stage_tab, stab.size() * sizeof(CtaStage)));
     CK(cudaMemcpy(h->chunk_tab, tab.data(), tab.size() * sizeof(ChunkDesc), cudaMemcpyHostToDevice));
     CK(cudaMemcpy(h->chunk_off, off.data(), off.size() * sizeof(int), cudaMemcpyHostToDevice));
+    CK(cudaMemcpy(h->stage_tab, stab.data(), stab.size() * sizeof(CtaStage), cudaMemcpyHostToDevice));
     m.chunk_tab = h->chunk_tab;
     m.chunk_off = h->chunk_off;
-    std::vector<CtaStage> stab;
-    dec_build_stage_table(m, h->ln_fold, h->n_cta, h->hi.cluster, stab);
-    if (h->stage_tab) { cudaFree(h->stage_tab); h->stage_tab = nullptr; }
-    CK(cudaMalloc((void**)&h->stage_tab, stab.size() * sizeof(CtaStage)));
-    CK(cudaMemcpy(h->stage_tab, stab.data(), stab.size() * sizeof(CtaStage), cudaMemcpyHostToDevice));
     m.stage_tab = h->stage_tab;
   }
   CK(cudaMemcpy(h->dm, &m, sizeof m, cudaMemcpyHostToDevice));
@@ -545,10 +544,7 @@ extern "C" int wm_set_medusa_choices(wm_handle* h, const int32_t* choices, int32
     m.has_tree = 1; m.tree = h->tree; m.n_tree = t.n_tree;
   }
   h->hi.n_tree = m.n_tree;
-  for (auto& kv : h->graph_a) cudaGraphExecDestroy(kv.second);
-  h->graph_a.clear();
-  if (h->graph_b) { cudaGraphExecDestroy(h->graph_b); h->graph_b = nullptr; }
-  if (h->graph_tail) { cudaGraphExecDestroy(h->graph_tail); h->graph_tail = nullptr; }
+  drop_graphs(h);
   if (h->wready) return bind_weights(h);   // the stage records of the verify vocabulary projection carry the row count
   CK(cudaMemcpy(h->dm, &m, sizeof m, cudaMemcpyHostToDevice));
   return WM_OK;
@@ -805,6 +801,26 @@ static int get_graph(wm_handle* h, int phase, int T, cudaGraphExec_t* out, int64
   return WM_OK;
 }
 
+// Enqueue one speculative iteration in decode mode `mode` on h->stream; returns its kernel launches, or a WM_ERR_*
+// status (< 0).  The persistent kernels (modes 1, 2) run what the loop state asks for: the whole iteration, or sweep A of
+// a prefill chunk.  Graph mode (0) runs phases 0 .. last_phase (sweep A over `rows` rows, the tail, verify); its sweep-A
+// kernels return at once unless the state says the newest token is uncached.  profile: the ring kernel records its
+// stage timeline (whole iterations only: the timeline's rows are laid out for the full program).
+static int64_t enqueue_iteration(wm_handle* h, int mode, int rows, int last_phase, bool profile) {
+  if (mode == 1) { CK(dec_launch_iteration(h->dm, h->hi, h->stream)); return 1; }
+  if (mode == 2) { CK(dec_launch_iteration_ring(h->dm, h->hi, profile, h->stream)); return 1; }
+  int64_t n = 0;
+  for (int phase = 0; phase <= last_phase; ++phase) {
+    cudaGraphExec_t g = nullptr;
+    int64_t nl = 0;
+    const int r = get_graph(h, phase, phase == 0 ? rows : 1, &g, &nl);
+    if (r != WM_OK) return r;
+    CK(cudaGraphLaunch(g, h->stream));
+    n += nl;
+  }
+  return n;
+}
+
 extern "C" int wm_generate(wm_handle* h, const int32_t* prompt, int32_t n_prompt, const wm_gen_params* gp,
                            int32_t* out_ids, int32_t* n_out, int32_t* accept_lens, int32_t* n_iter) {
   if (!h || !prompt || !gp || !out_ids || !n_out) return WM_ERR_INVALID;
@@ -858,18 +874,9 @@ extern "C" int wm_generate(wm_handle* h, const int32_t* prompt, int32_t n_prompt
       DecState& hs = *h->h_init;
       hs.L = pos + WM_MAX_T; hs.kv_len = pos; hs.need_a = 1; hs.prefill = 1;
       CK(cudaMemcpyAsync(h->st, &hs, 64, cudaMemcpyHostToDevice, s));   // the 16 header words (L .. tree_attn)
-      if (h->decode_mode == 0) {
-        cudaGraphExec_t g = nullptr; int64_t nl = 0; int r;
-        if ((r = get_graph(h, 0, WM_MAX_T, &g, &nl)) != WM_OK) return r;
-        CK(cudaGraphLaunch(g, s));
-        h->launches[2] += nl;
-      } else if (h->decode_mode == 1) {
-        CK(dec_launch_iteration(h->dm, h->hi, s));
-        h->launches[2] += 1;
-      } else {
-        CK(dec_launch_iteration_ring(h->dm, h->hi, false, s));
-        h->launches[2] += 1;
-      }
+      const int64_t nl = enqueue_iteration(h, h->decode_mode, WM_MAX_T, 0, false);
+      if (nl < 0) return (int)nl;
+      h->launches[2] += nl;
       CK(cudaStreamSynchronize(s));   // the pinned header is rewritten for the next chunk
       pos += WM_MAX_T;
     }
@@ -880,14 +887,16 @@ extern "C" int wm_generate(wm_handle* h, const int32_t* prompt, int32_t n_prompt
       n_tail = n_prompt - pos;
     }
   }
-  cudaGraphExec_t gA1 = nullptr, gAp = nullptr, gT = nullptr, gB = nullptr;
-  int64_t nA1 = 0, nAp = 0, nT = 0, nB = 0;
   if (h->decode_mode == 0) {
-    int r;
-    if ((r = get_graph(h, 0, n_tail, &gAp, &nAp)) != WM_OK) return r;
-    if ((r = get_graph(h, 0, 1, &gA1, &nA1)) != WM_OK) return r;
-    if ((r = get_graph(h, 1, 1, &gT, &nT)) != WM_OK) return r;
-    if ((r = get_graph(h, 2, h->hm.n_tree, &gB, &nB)) != WM_OK) return r;
+    // capture the graphs of this call before the timed loop ({phase, rows}: the rows only key the sweep-A graphs; there
+    // is one tail and one verify graph, and the verify rows come from n_tree)
+    const int need[4][2] = {{0, n_tail}, {0, 1}, {1, 1}, {2, 1}};
+    for (const auto& p : need) {
+      cudaGraphExec_t g = nullptr;
+      int64_t nl = 0;
+      const int r = get_graph(h, p[0], p[1], &g, &nl);
+      if (r != WM_OK) return r;
+    }
   }
   CK(cudaEventRecord(h->ev[3], s));
   int L = n_prompt, iters = 0, done = 0;
@@ -900,20 +909,9 @@ extern "C" int wm_generate(wm_handle* h, const int32_t* prompt, int32_t n_prompt
     if (gp->max_iters > 0 && lb > gp->max_iters - iters) lb = gp->max_iters - iters;
     if (lb < 1) lb = 1;
     for (int i = 0; i < lb; ++i) {
-      if (h->decode_mode == 0) {
-        const bool first = (iters + i == 0);
-        // sweep A kernels return immediately unless the state says the newest token is uncached
-        CK(cudaGraphLaunch(first ? gAp : gA1, s));
-        CK(cudaGraphLaunch(gT, s));
-        CK(cudaGraphLaunch(gB, s));
-        h->launches[2] += (first ? nAp : nA1) + nT + nB;
-      } else if (h->decode_mode == 1) {
-        CK(dec_launch_iteration(h->dm, h->hi, s));
-        h->launches[2] += 1;
-      } else {
-        CK(dec_launch_iteration_ring(h->dm, h->hi, h->hm.prof != nullptr, s));
-        h->launches[2] += 1;
-      }
+      const int64_t nl = enqueue_iteration(h, h->decode_mode, iters + i == 0 ? n_tail : 1, 2, h->hm.prof != nullptr);
+      if (nl < 0) return (int)nl;
+      h->launches[2] += nl;
     }
     CK(cudaMemcpyAsync(h->h_state, h->st, 16 * sizeof(int), cudaMemcpyDeviceToHost, s));
     CK(cudaStreamSynchronize(s));
@@ -968,21 +966,14 @@ extern "C" int wm_forward(wm_handle* h, const int32_t* ids, int32_t n_ids, float
     CK(cudaMemcpyAsync(h->st, &hs, sizeof hs, cudaMemcpyHostToDevice, s));
     CK(cudaMemsetAsync(h->hm.cross_cnt, 0, (size_t)h->cfg.n_heads * sizeof(unsigned int), s));
     CK(cudaMemsetAsync(h->hm.gemm_cnt, 0, (size_t)h->n_sm * sizeof(unsigned int), s));
-    if (h->decode_mode == 2) {
-      // ring kernel (any decode grid): one speculative iteration = sweep A over the prefix, the candidate tail (whose
-      // K+1 logit rows are what we want) and a verify pass whose results are simply not read
-      CK(cudaMemsetAsync(h->bar, 0, 8 * sizeof(unsigned int), s));
-      CK(dec_launch_iteration_ring(h->dm, h->hi, false, s));
-    } else {
-      if (!simple_modes_fit(h)) return fail(h, WM_ERR_UNSUPPORTED, "wm_forward: this decode grid needs the ring kernel (decode_mode 2)");
-      cudaGraphExec_t gA = nullptr, gT = nullptr;
-      int64_t nA = 0, nT = 0;
-      int r;
-      if ((r = get_graph(h, 0, t, &gA, &nA)) != WM_OK) return r;
-      if ((r = get_graph(h, 1, 1, &gT, &nT)) != WM_OK) return r;
-      CK(cudaGraphLaunch(gA, s));
-      CK(cudaGraphLaunch(gT, s));
-    }
+    // sweep A over the prefix and the candidate tail, whose K+1 logit rows are what we want.  The ring kernel (any decode
+    // grid) runs them as one speculative iteration whose verify pass is simply not read; the other modes run the two
+    // graphs alone.
+    const bool ring = h->decode_mode == 2;
+    if (ring) CK(cudaMemsetAsync(h->bar, 0, 8 * sizeof(unsigned int), s));
+    else if (!simple_modes_fit(h)) return fail(h, WM_ERR_UNSUPPORTED, "wm_forward: this decode grid needs the ring kernel (decode_mode 2)");
+    const int64_t nl = enqueue_iteration(h, ring ? 2 : 0, t, 1, false);
+    if (nl < 0) return (int)nl;
     for (int k = 0; k <= K; ++k)
       CK(cudaMemcpyAsync(out + ((size_t)k * n_ids + (t - 1)) * V, h->hm.logits_a + (size_t)k * V, V * sizeof(float),
                          cudaMemcpyDeviceToHost, s));
@@ -1044,10 +1035,7 @@ extern "C" int wm_set_option(wm_handle* h, const char* key, int32_t value) {
     h->hi.n_sm = value;
     h->hi.cluster = dec_ring_cluster_size(h->hi, h->n_sm);
     set_decode_split(h);
-    for (auto& kv : h->graph_a) cudaGraphExecDestroy(kv.second);
-    h->graph_a.clear();
-    if (h->graph_b) { cudaGraphExecDestroy(h->graph_b); h->graph_b = nullptr; }
-    if (h->graph_tail) { cudaGraphExecDestroy(h->graph_tail); h->graph_tail = nullptr; }
+    drop_graphs(h);
     if (!simple_modes_fit(h)) {
       if (!h->hi.smem_ring) return fail(h, WM_ERR_UNSUPPORTED, "too few CTAs for this model without the ring kernel");
       h->decode_mode = 2;
@@ -1057,7 +1045,7 @@ extern "C" int wm_set_option(wm_handle* h, const char* key, int32_t value) {
     return WM_OK;
   }
   if (k == "profile") {
-    // stage timeline of the persistent ring kernel (debug): buffer [2][n_instr][3] u64
+    // stage timeline of the persistent ring kernel (debug): buffer [2][n_instr][16] u64
     CK(cudaSetDevice(h->device));
     if (value && !h->prof) CK(dalloc(&h->prof, (size_t)2 * h->hm.prog_off[3] * 16));
     h->hm.prof = value ? h->prof : nullptr;
@@ -1095,16 +1083,14 @@ extern "C" int wm_get_stage_profile(wm_handle* h, int64_t* out, int32_t cap_rows
   CK(cudaSetDevice(h->device));
   const int n = h->hm.prog_off[3];
   std::vector<unsigned long long> raw((size_t)2 * n * 16);
-  std::vector<int> prog((size_t)n * 3);
   CK(cudaMemcpy(raw.data(), h->prof, raw.size() * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
-  CK(cudaMemcpy(prog.data(), h->prog, prog.size() * sizeof(int), cudaMemcpyDeviceToHost));
   int rows = 0;
   for (int i = 0; i < n && rows < cap_rows; ++i) {
     const unsigned long long* a = &raw[(size_t)i * 16];
     const unsigned long long* b = &raw[((size_t)n + i) * 16];
     if (a[0] == 0) continue;   // stage never executed (sweep A skipped)
     int64_t* o = out + (size_t)rows * 24;
-    o[0] = prog[i * 3]; o[1] = prog[i * 3 + 1]; o[2] = prog[i * 3 + 2];
+    o[0] = h->prog[i * 3]; o[1] = h->prog[i * 3 + 1]; o[2] = h->prog[i * 3 + 2];
     o[3] = (int64_t)(b[1] - b[0]); o[4] = (int64_t)(b[2] - b[1]);
     for (int k = 0; k < 16; ++k) {
       const bool flag = (k == 11 || k == 12);

@@ -25,8 +25,6 @@ size_t dec_smem_bytes(int d, int ffn);
 cudaError_t dec_configure(int d, size_t smem, size_t smem_ring);
 size_t dec_ring_smem_bytes(int d);
 void dec_build_program(int n_layers, int has_block, std::vector<int>& flat, int off[4]);
-struct ChunkDesc;
-void dec_build_chunk_table(const DecModel& hm, int ncta, std::vector<ChunkDesc>& tab, std::vector<int>& off);
 cudaError_t dec_relayout_cross_kv(const __half* kv, __half* ck, __half* cv, int S, int S_pad, int d, int H, cudaStream_t s,
                                   int64_t* n_launch);
 // {b'_n, c_n} of the LayerNorm-fed GEMMs of the ring kernel: float2 count for n_dec decoder layers, and the derivation
@@ -34,7 +32,11 @@ cudaError_t dec_relayout_cross_kv(const __half* kv, __half* ck, __half* cv, int 
 size_t dec_ln_fold_len(int n_dec, int d, int ffn);
 cudaError_t dec_fold_layernorms(const DecModel& hm, int n_dec, float2* out, cudaStream_t s);
 struct CtaStage;
-void dec_build_stage_table(const DecModel& hm, const float2* ln_fold, int ncta, int cluster, std::vector<CtaStage>& tab);
+struct ChunkDesc;
+// the ring kernel's stage records [instruction][cta] and per-CTA chunk schedule (chunk_off: 4 per CTA), for a grid of
+// ncta CTAs in clusters of `cluster`
+void dec_build_ring_tables(const DecModel& hm, const float2* ln_fold, int ncta, int cluster, std::vector<CtaStage>& stab,
+                           std::vector<ChunkDesc>& ctab, std::vector<int>& off);
 cudaError_t dec_launch_iteration_ring(const DecModel* dm, const DecHostInfo& hi, bool profile, cudaStream_t s);
 int dec_ring_cluster_size(const DecHostInfo& hi, int n_sm);
 // phase: 0 = sweep A over T uncached rows, 1 = tail (candidates), 2 = verify sweep + accept
