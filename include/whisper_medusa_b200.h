@@ -135,6 +135,16 @@ int wm_resample_taps(int32_t orig_hz, int32_t new_hz, float* taps, int32_t* lo, 
  * accept_lens (capacity >= max_length, may be NULL) receives the per-iteration accept length. */
 int wm_generate(wm_handle* h, const int32_t* prompt, int32_t n_prompt, const wm_gen_params* gp,
                 int32_t* out_ids, int32_t* n_out, int32_t* accept_lens, int32_t* n_iter);
+/* What the last wm_generate scored (option "scores", set before the call; model.py:737-742 output_scores / output_logits).
+ * Rows are processed with cur_len = len(input_ids) at the start of their iteration (suppress, begin-suppress, EOS decay).
+ * token_logprobs (capacity cap): log_softmax at temperature 1 of the row each generated token was chosen from, one per
+ * position after the prompt (*n_tokens = n_out - n_prompt): the first token of an iteration from the base row of the
+ * tail, the j-th from verify row path[j - 1] of the best candidate.  Needs bit 0.
+ * rows (capacity cap_rows rows of vocab_size floats): per iteration the processed verify row path[accept]
+ * (medusa_utils.py:663-664 next_token_logits), *n_rows = iterations.  Needs bit 1.
+ * Either output may be NULL.  WM_ERR_STATE if the last wm_generate did not record what is asked for. */
+int wm_last_scores(wm_handle* h, float* token_logprobs, int32_t cap, int32_t* n_tokens, float* rows, int32_t cap_rows,
+                   int32_t* n_rows);
 
 /* ---- teacher-forced forward (model.py:1223-1347 `forward(...).logits`, shape [K+1, 1, T, V]) -------------- */
 /* ids: 1..16 decoder_input_ids; out (host, capacity (K+1) * n_ids * vocab_size floats) receives the raw logits of
@@ -170,7 +180,8 @@ void* wm_weights_device_ptr(wm_handle* h);
  * 0 = mma.sync encoder GEMM (cross-check), 2 = wgmma with 128 x 128 tiles only (cross-check of the per-GEMM tile
  * shapes); "enc_attn" 1 = wgmma/TMA encoder attention (default), 0 = mma.sync flash attention (cross-check);
  * "enc_pdl" 1 = encoder kernels under programmatic dependent launch (default), 0 = plain stream-ordered launches;
- * "profile" 1 = record the stage timeline below. */
+ * "profile" 1 = record the stage timeline below; "scores" = what wm_generate records for wm_last_scores: bit 0 the
+ * per-token log-probabilities, bit 1 the scores rows (0, the default: nothing, and no extra launch). */
 int wm_set_option(wm_handle* h, const char* key, int32_t value);
 /* Host logic, no GPU needed: the tile {rows, columns, ring stages} the wgmma encoder GEMM runs an M x N x K product
  * with on a GPU of n_sm SMs (0: 132) -- the shape with the fewest operand bytes on the busiest SM (DESIGN.md section 4).

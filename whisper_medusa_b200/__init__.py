@@ -4,7 +4,8 @@
 ``from whisper_medusa import WhisperMedusaModel`` (reference ``whisper_medusa/__init__.py:1``).
 """
 from .config import MedusaConfig, MedusaGenerationConfig  # noqa: F401
-from .model import EngineError, WhisperMedusaModel  # noqa: F401
+from .model import EngineError, MedusaGenerateOutput, WhisperMedusaModel  # noqa: F401
 from .streams import StreamGroup  # noqa: F401
 
-__all__ = ["WhisperMedusaModel", "StreamGroup", "MedusaConfig", "MedusaGenerationConfig", "EngineError"]
+__all__ = ["WhisperMedusaModel", "StreamGroup", "MedusaConfig", "MedusaGenerationConfig", "EngineError",
+           "MedusaGenerateOutput"]

@@ -221,7 +221,20 @@ struct DecState {
   int row_argmax[WM_MAX_T];
   float row_pc[WM_MAX_T];        // [n]: softmax prob of node n's token in the posterior of its parent row (chain: parent = n-1)
   float row_thr[WM_MAX_T];
+  int path_node;    // tree mode: node path[accept] of the best candidate of the last iteration (read by the scoring kernel)
 };
+
+// Logits processors applied to element j of a raw logits row, with cur_len = L (HF logits_process.py:1893-1901 suppress,
+// :1847-1862 begin-suppress when L == begin_index, :1742-1772 EOS exponential decay with pen = pen_tab[L]).  Shared by
+// the loop's logits scan and the scoring kernel.
+__device__ __forceinline__ float processed_logit(const float* row, int j, const uint8_t* mask, bool begin_on,
+                                                 int eos, float pen) {
+  const uint8_t mk = mask[j];
+  if ((mk & 1) || (begin_on && (mk & 2))) return -INFINITY;
+  float v = ldcg_f(row + j);
+  if (j == eos && pen != 0.f) v = v + fabsf(v) * pen;
+  return v;
+}
 
 struct alignas(16) DecModel {   // (copied to shared memory in 16-byte pieces by the ring kernel)
   int d, H, ffn, V, S, S_pad;

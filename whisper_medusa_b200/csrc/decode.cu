@@ -813,15 +813,6 @@ __device__ void stage_tail_seed(const DecModel* m, int cta, int ncta) {
 //   pass A: generate_candidates with top-1 per head (medusa_utils.py:446-457)
 //   pass B: evaluate_posterior (medusa_utils.py:547-588)
 // -----------------------------------------------------------------------------------------
-__device__ __forceinline__ float processed_logit(const float* row, int j, const uint8_t* mask, bool begin_on,
-                                                 int eos, float pen) {
-  const uint8_t mk = mask[j];
-  if ((mk & 1) || (begin_on && (mk & 2))) return -INFINITY;
-  float v = ldcg_f(row + j);
-  if (j == eos && pen != 0.f) v = v + fabsf(v) * pen;
-  return v;
-}
-
 __device__ void block_argmax(float& v, int& i, float* s_val, int* s_idx) {
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = (WM_DEC_THREADS >> 5);
 #pragma unroll
@@ -1209,6 +1200,7 @@ __device__ __noinline__ void stage_accept_tree(const DecModel* m, int ncta) {
       if (done) st->done = 1;
       s_a = elide ? a : -1;
       s_node = tr->retrieve[best][a];
+      st->path_node = s_node;
     }
   }
   cta_sync();

@@ -100,6 +100,13 @@ struct wm_handle {
     size_t smem = 0;
   };
   std::map<std::pair<int, int>, Resampler> resamplers;
+  // scoring (option "scores": bit 0 per-token log-probabilities, bit 1 scores rows); buffers allocated on first use
+  int score_bits = 0;
+  int* score_state = nullptr;   // {iterations scored, cursor, arrivals}
+  float* score_part = nullptr;  // segment partials of the rows being scored
+  float* score_lp = nullptr;    // [WM_MAX_POS + 32] log-probability per position
+  float* score_rows = nullptr;  // [max_target_positions][V] scores rows
+  int last_score_bits = 0, last_prompt = 0, last_L = 0, last_iters = 0;   // what the last wm_generate scored
 };
 
 static_assert(offsetof(DecState, tree_attn) == 60, "the 16 header words of DecState (L .. tree_attn) are patched as one 64-byte copy");
@@ -380,6 +387,7 @@ extern "C" int wm_destroy(wm_handle* h) {
   for (auto p : h->self_v) F(p);
   F(h->hm.x); F(h->hm.xg); F(h->hm.q); F(h->hm.attn); F(h->hm.ffn_h); F(h->hm.hidden); F(h->hm.head_h); F(h->hm.carry); F(h->hm.cross_part); F(h->hm.cross_cnt); F(h->hm.sel_part); F(h->hm.gemm_part); F(h->hm.gemm_cnt);
   F(h->hm.topk_part); F(h->tree); F(h->hm.logits_a); F(h->hm.logits_b); F(h->st); F(h->tok_mask); F(h->pen_tab); F(h->bar); F(h->prof); F(h->chunk_tab); F(h->chunk_off); F(h->stage_tab); F(h->ln_fold); F(h->dm);
+  F(h->score_state); F(h->score_part); F(h->score_lp); F(h->score_rows);
   if (h->wowned) F(h->wdev);
   for (auto& kv : h->resamplers) { F(kv.second.taps); F(kv.second.sup); }
   if (h->h_state) cudaFreeHost(h->h_state);
@@ -834,6 +842,7 @@ extern "C" int wm_generate(wm_handle* h, const int32_t* prompt, int32_t n_prompt
   CK(cudaSetDevice(h->device));
   cudaStream_t s = h->stream;
   h->launches[2] = 0;
+  h->last_score_bits = 0;
 
   // EOS exponential-decay penalty table (HF logits_process.py:1742-1772): indexed by cur_len
   if (gp->penalty_start != h->last_pen_start || gp->penalty_factor != h->last_pen_factor || n_prompt != h->last_pen_prompt) {
@@ -865,6 +874,16 @@ extern "C" int wm_generate(wm_handle* h, const int32_t* prompt, int32_t n_prompt
     CK(cudaMemsetAsync(h->hm.cross_cnt, 0, (size_t)h->cfg.n_heads * sizeof(unsigned int), s));
     CK(cudaMemsetAsync(h->hm.gemm_cnt, 0, (size_t)h->n_sm * sizeof(unsigned int), s));
   }
+  const int score_bits = h->score_bits;
+  if (score_bits) CK(cudaMemsetAsync(h->score_state, 0, 4 * sizeof(int), s));
+  ScoreArgs sa;
+  memset(&sa, 0, sizeof sa);
+  sa.logits_a = h->hm.logits_a; sa.logits_b = h->hm.logits_b; sa.st = h->st; sa.tree = h->hm.has_tree ? h->tree : nullptr;
+  sa.tok_mask = h->tok_mask; sa.pen_tab = h->pen_tab; sa.V = h->cfg.vocab_size; sa.n_prompt = n_prompt;
+  sa.want_lp = score_bits & 1; sa.want_rows = (score_bits >> 1) & 1;
+  sa.state = h->score_state; sa.part = h->score_part; sa.lp = h->score_lp; sa.rows = h->score_rows;
+  sa.cap_rows = h->cfg.max_target_positions;
+  const int score_grid = dec_score_grid(h->n_cta, K);
   // Long prompts (decoder_input_ids beyond the 16 rows of a stage tile): the leading tokens are cached by prefill
   // launches -- sweep A over 16-token chunks, no candidates / verify -- before the loop proper starts on the rest.
   int n_tail = n_prompt;     // rows of the first real iteration's sweep A
@@ -912,6 +931,10 @@ extern "C" int wm_generate(wm_handle* h, const int32_t* prompt, int32_t n_prompt
       const int64_t nl = enqueue_iteration(h, h->decode_mode, iters + i == 0 ? n_tail : 1, 2, h->hm.prof != nullptr);
       if (nl < 0) return (int)nl;
       h->launches[2] += nl;
+      if (score_bits) {   // reads what the iteration left behind; a no-op once the loop has ended
+        CK(dec_launch_scores(sa, score_grid, s));
+        h->launches[2] += 1;
+      }
     }
     CK(cudaMemcpyAsync(h->h_state, h->st, 16 * sizeof(int), cudaMemcpyDeviceToHost, s));
     CK(cudaStreamSynchronize(s));
@@ -940,6 +963,29 @@ extern "C" int wm_generate(wm_handle* h, const int32_t* prompt, int32_t n_prompt
   if (accept_lens && iters > 0)
     CK(cudaMemcpy(accept_lens, reinterpret_cast<const char*>(h->st) + offsetof(DecState, accept_hist),
                   (size_t)iters * sizeof(int), cudaMemcpyDeviceToHost));
+  h->last_score_bits = score_bits; h->last_prompt = n_prompt; h->last_L = L; h->last_iters = iters;
+  return WM_OK;
+}
+
+extern "C" int wm_last_scores(wm_handle* h, float* token_logprobs, int32_t cap, int32_t* n_tokens, float* rows,
+                              int32_t cap_rows, int32_t* n_rows) {
+  if (!h) return WM_ERR_INVALID;
+  if ((token_logprobs && cap < 0) || (rows && cap_rows < 0)) return WM_ERR_INVALID;
+  if ((token_logprobs || n_tokens) && !(h->last_score_bits & 1))
+    return fail(h, WM_ERR_STATE, "the last wm_generate did not record log-probabilities (option \"scores\" bit 0)");
+  if ((rows || n_rows) && !(h->last_score_bits & 2))
+    return fail(h, WM_ERR_STATE, "the last wm_generate did not record scores rows (option \"scores\" bit 1)");
+  CK(cudaSetDevice(h->device));
+  const int nt = h->last_L - h->last_prompt;
+  const int nr = std::min(h->last_iters, h->cfg.max_target_positions);
+  if (n_tokens) *n_tokens = nt;
+  if (n_rows) *n_rows = nr;
+  if (token_logprobs && std::min(cap, nt) > 0)
+    CK(cudaMemcpy(token_logprobs, h->score_lp + h->last_prompt, (size_t)std::min(cap, nt) * sizeof(float),
+                  cudaMemcpyDeviceToHost));
+  if (rows && std::min(cap_rows, nr) > 0)
+    CK(cudaMemcpy(rows, h->score_rows, (size_t)std::min(cap_rows, nr) * h->cfg.vocab_size * sizeof(float),
+                  cudaMemcpyDeviceToHost));
   return WM_OK;
 }
 
@@ -1050,6 +1096,22 @@ extern "C" int wm_set_option(wm_handle* h, const char* key, int32_t value) {
     if (value && !h->prof) CK(dalloc(&h->prof, (size_t)2 * h->hm.prog_off[3] * 16));
     h->hm.prof = value ? h->prof : nullptr;
     CK(cudaMemcpy(h->dm, &h->hm, sizeof(DecModel), cudaMemcpyHostToDevice));
+    return WM_OK;
+  }
+  if (k == "scores") {
+    // bit 0: log-probability of every generated token; bit 1: the scores row of every iteration (wm_last_scores).
+    // Off (0) by default: the loop then launches exactly what it launches without scoring.
+    if (value < 0 || value > 3) return fail(h, WM_ERR_INVALID, "scores must be 0..3 (bit 0 log-probabilities, bit 1 rows)");
+    if (h->device < 0) return fail(h, WM_ERR_STATE, "layout-only handle");
+    CK(cudaSetDevice(h->device));
+    if (value && !h->score_state) {
+      CK(dalloc(&h->score_state, 4));
+      CK(dalloc(&h->score_part, (size_t)(WM_MAX_T + 1) * (WM_SCORE_NSEG * 2 + 1)));
+      CK(dalloc(&h->score_lp, (size_t)WM_MAX_POS + 32));
+    }
+    if ((value & 2) && !h->score_rows)
+      CK(dalloc(&h->score_rows, (size_t)h->cfg.max_target_positions * h->cfg.vocab_size));
+    h->score_bits = value;
     return WM_OK;
   }
   if (k == "enc_attn") {

@@ -43,6 +43,32 @@ int dec_ring_cluster_size(const DecHostInfo& hi, int n_sm);
 cudaError_t dec_enqueue_phase(const DecModel* dm, const DecHostInfo& hi, int phase, int T, cudaStream_t s, int64_t* n_launch);
 cudaError_t dec_launch_iteration(const DecModel* dm, const DecHostInfo& hi, cudaStream_t s);
 
+// ---- scores.cu ----
+#define WM_SCORE_NSEG 16       // vocabulary segments per scored row (fixed: the fold order does not depend on the grid)
+#define WM_SCORE_THREADS 512
+#define WM_SCORE_UNROLL 4      // elements per thread loaded together (one segment of large-v2's vocabulary: 2 steps)
+struct DecState;
+struct DecTree;
+// What the scoring kernel reads and writes; one launch after each speculative iteration while scoring is on.
+struct ScoreArgs {
+  const float* logits_a;   // [K+1][V] raw rows of the tail (row 0: the base row c0 was chosen from)
+  const float* logits_b;   // [n_tree][V] raw verify rows
+  const DecState* st;
+  const DecTree* tree;     // null for a chain
+  const uint8_t* tok_mask;
+  const float* pen_tab;
+  int V;
+  int n_prompt;            // first position scored (prefill launches of a long prompt are not scored)
+  int want_lp, want_rows;  // option "scores" bit 0 / bit 1
+  int* state;              // {iterations scored, cursor = first unscored position, arrivals}; zero at the start of a call
+  float* part;             // [WM_MAX_T + 1][WM_SCORE_NSEG]{max, sum of exp(v - max)}, then [WM_MAX_T + 1] token logits
+  float* lp;               // [WM_MAX_POS + 32]: log-probability of the token at each position
+  float* rows;             // [cap_rows][V]: processed verify row path[accept] of each iteration
+  int cap_rows;
+};
+int dec_score_grid(int n_cta, int K);
+cudaError_t dec_launch_scores(const ScoreArgs& a, int grid, cudaStream_t s);
+
 // ---- mel.cu ----
 // pcm: device f32 [480000] (already zero padded). Outputs: mel_f32 [80][3000], xT fp16 [rows>=3000+?][80]
 // time-major with one leading zero row (conv padding); gmax_bits: device scratch (1 int).

@@ -8,7 +8,10 @@ Same names, argument meaning and error behaviour as the reference for this path:
 * ``return_timestamps`` -> ``NotImplementedError`` (``:1171-1174``); ``no_speech_threshold`` ->
   ``NotImplementedError`` (``:1201-1204``); more than 3000 feature frames (long-form) ->
   ``NotImplementedError`` (``:1213-1214``); beam search -> ``Exception`` (``:1153-1156``);
-* the returned ``LongTensor[1, n]`` has the prompt and the trailing EOS stripped (``:1929-1973``).
+* the returned ``LongTensor[1, n]`` has the prompt and the trailing EOS stripped (``:1929-1973``);
+* ``return_dict_in_generate=True`` with ``output_scores`` / ``output_logits`` returns the per-iteration processed rows the
+  reference collects (``:737-742``) in a ``MedusaGenerateOutput``, with per-token log-probabilities added (computed on the
+  GPU, ``csrc/scores.cu``).
 
 Beyond the reference (which takes 16 kHz clips of at most 30 s): ``transcribe`` takes a recording of any length at any
 integer sampling rate, with the semantics of HF's chunked ASR pipeline (``longform.py``); ``generate_from_pcm`` takes
@@ -98,6 +101,48 @@ class ForwardOutput:
         if i in (0, "logits"):
             return self.logits
         raise KeyError(i)
+
+
+class MedusaGenerateOutput:
+    """What ``generate(..., return_dict_in_generate=True)`` returns (the reference returns a
+    ``GenerateEncoderDecoderOutput``, ``model.py:812-824``).
+
+    * ``sequences``: ``LongTensor[1, n]``, exactly what the call returns without ``return_dict_in_generate``;
+    * ``scores`` (``output_scores=True``, else ``None``): one ``FloatTensor[1, V]`` per speculative iteration, the
+      processed verify row of the accepted path's last node (the reference's ``next_token_logits``, whose own shape is
+      ``[1, 1, V]``); suppressed ids are ``-inf``;
+    * ``logits`` (``output_logits=True``, else ``None``): the same rows (the reference appends the same processed tensor
+      to both tuples, ``model.py:739-742``);
+    * ``token_logprobs``: ``FloatTensor[1, n_new_tokens]``, the log-probability (log_softmax at temperature 1 of the
+      processed row) of every generated token up to and including the first EOS, under the row it was chosen from;
+    * ``avg_logprob``: their mean (a float);
+    * ``accept_lengths``: the accept length of every iteration.
+
+    Fields are attributes and keys (``out.scores`` / ``out["scores"]``); an integer indexes the fields that are not
+    ``None``, in the order above, as HF ``ModelOutput`` does."""
+
+    FIELDS = ("sequences", "scores", "logits", "token_logprobs", "avg_logprob", "accept_lengths")
+
+    def __init__(self, sequences, scores, logits, token_logprobs, avg_logprob, accept_lengths):
+        self.sequences = sequences
+        self.scores = scores
+        self.logits = logits
+        self.token_logprobs = token_logprobs
+        self.avg_logprob = avg_logprob
+        self.accept_lengths = accept_lengths
+
+    def keys(self) -> List[str]:
+        return [k for k in self.FIELDS if getattr(self, k) is not None]
+
+    def to_tuple(self) -> tuple:
+        return tuple(getattr(self, k) for k in self.keys())
+
+    def __getitem__(self, i):
+        if isinstance(i, str):
+            if i not in self.FIELDS:
+                raise KeyError(i)
+            return getattr(self, i)
+        return self.to_tuple()[i]
 
 
 class GenerateTrace:
@@ -390,9 +435,11 @@ class WhisperMedusaModel:
                  condition_on_prev_tokens=None, temperature=None, compression_ratio_threshold=None,
                  logprob_threshold=None, no_speech_threshold=None, num_segment_frames=None, attention_mask=None,
                  time_precision: float = 0.02, return_token_timestamps=None, return_segments: bool = False,
-                 return_dict_in_generate=None, **kwargs) -> torch.Tensor:
+                 return_dict_in_generate=None, **kwargs) -> Union[torch.Tensor, MedusaGenerateOutput]:
         """Transcribe one <= 30 s clip given its log-mel features ``[1, 80, 3000]``
-        (reference ``model.py:1419-1779``); returns ``LongTensor[1, n]``."""
+        (reference ``model.py:1419-1779``); returns ``LongTensor[1, n]``, or with ``return_dict_in_generate=True`` a
+        ``MedusaGenerateOutput`` (``output_scores`` / ``output_logits`` select its ``scores`` / ``logits``; without
+        ``return_dict_in_generate`` they have no effect, as in HF and the reference)."""
         self._require_engine()
         if input_features is None:
             raise ValueError("input_features is required")
@@ -413,7 +460,7 @@ class WhisperMedusaModel:
             raise ValueError(f"input_features must be [1, {self.config.num_mel_bins}, {N_FRAMES}] (WhisperProcessor output)")
         self._check_unsupported(temperature, attention_mask, kwargs)
         self._encode_features(input_features)
-        return self._decode(language, task, kwargs, temperature, generation_config)
+        return self._decode(language, task, kwargs, temperature, generation_config, return_dict_in_generate)
 
     def _encode_features(self, input_features: torch.Tensor) -> None:
         lib = _lib.load()
@@ -441,14 +488,14 @@ class WhisperMedusaModel:
             raise NotImplementedError("sampling (temperature > 0 / do_sample) is not supported with medusa: greedy search only")
         known = {"exponential_decay_length_penalty", "max_length", "max_new_tokens", "max_iters", "medusa_temperature",
                  "posterior_threshold", "posterior_alpha", "num_beams", "do_sample", "use_cache", "tree_attention",
-                 "decoder_input_ids"}
+                 "decoder_input_ids", "output_scores", "output_logits"}
         unknown = sorted(set(kwargs) - known)
         if unknown:
             raise NotImplementedError(f"generate() options not implemented by the H100 engine: {unknown}")
 
     def generate_from_pcm(self, pcm: Union[np.ndarray, torch.Tensor], language: Optional[str] = None,
                           task: Optional[str] = None, temperature=None, sampling_rate: int = SAMPLE_RATE,
-                          **kwargs) -> torch.Tensor:
+                          return_dict_in_generate=None, **kwargs) -> Union[torch.Tensor, MedusaGenerateOutput]:
         """Same as ``generate`` but takes mono f32 PCM and runs the log-mel frontend on the GPU
         (what ``WhisperProcessor`` does on the CPU in the reference's caller, eval_whisper_medusa.py:46-51).
         ``sampling_rate`` other than 16000 (any positive integer rate): the clip is uploaded and resampled to 16 kHz on
@@ -461,7 +508,7 @@ class WhisperMedusaModel:
             self._check_unsupported(temperature, None, kwargs)
             x16 = self._upload_16k(x, sampling_rate)
             self._encode_window(x16, Window(0, x16.numel(), 0, 0), torch.cuda.current_stream(self._device).cuda_stream)
-            return self._decode(language, task, kwargs, temperature)
+            return self._decode(language, task, kwargs, temperature, return_dict_in_generate=return_dict_in_generate)
         x = torch.as_tensor(pcm).detach().to("cpu", torch.float32).contiguous().reshape(-1)
         if x.numel() > 480000:
             raise NotImplementedError("Longform generation is not supported yet")
@@ -470,7 +517,7 @@ class WhisperMedusaModel:
                lib.wm_encode_pcm(self._handle, C.cast(x.data_ptr(), C.POINTER(C.c_float)), int(x.numel())),
                "wm_encode_pcm")
         self._check_unsupported(temperature, None, kwargs)
-        return self._decode(language, task, kwargs, temperature)
+        return self._decode(language, task, kwargs, temperature, return_dict_in_generate=return_dict_in_generate)
 
     # ------------------------------------------------------------------ long-form (HF chunked ASR pipeline)
     def transcribe(self, audio: Union[np.ndarray, torch.Tensor], sampling_rate: int = SAMPLE_RATE,
@@ -541,8 +588,15 @@ class WhisperMedusaModel:
         ids = self._decode(language, task, kwargs, temperature)[0].tolist()
         return WindowResult(w, ids, self.last_trace)
 
-    def _decode(self, language, task, kwargs, temperature, generation_config=None) -> torch.Tensor:
+    def _decode(self, language, task, kwargs, temperature, generation_config=None,
+                return_dict_in_generate=None) -> Union[torch.Tensor, MedusaGenerateOutput]:
         g = generation_config if generation_config is not None else self.generation_config
+        output_scores = bool(kwargs.pop("output_scores", False))
+        output_logits = bool(kwargs.pop("output_logits", False))
+        as_dict = bool(return_dict_in_generate)
+        # engine option "scores" for this call: bit 0 = per-token log-probabilities (every dict result), bit 1 = the
+        # scores rows.  0 without return_dict_in_generate: the loop then launches nothing extra.
+        score_bits = (1 | (2 if output_scores or output_logits else 0)) if as_dict else 0
         cur = (tuple(g.suppress_tokens or []), tuple(g.begin_suppress_tokens or []))
         if cur != getattr(self, "_pushed", None):
             self._push_suppress()
@@ -569,10 +623,44 @@ class WhisperMedusaModel:
         # branching medusa_choices: False (default) = the reference's behaviour (its medusa_attn_mask is built but never
         # applied: verify rows attend causally over cache order); True = every node attends to its ancestors only
         gp.tree_attention = 1 if kwargs.pop("tree_attention", False) else 0
+        lib = _lib.load()
+        _check(lib, self._handle, lib.wm_set_option(self._handle, b"scores", score_bits), "wm_set_option(scores)")
         tr = self._run_loop(prompt, gp)
         self.last_trace = tr
         out = self._strip(tr.sequences, len(prompt), int(gp.pad_token_id), int(gp.eos_token_id))
-        return torch.tensor([out], dtype=torch.long, device=self._device)
+        sequences = torch.tensor([out], dtype=torch.long, device=self._device)
+        if not as_dict:
+            return sequences
+        return self._generate_output(sequences, tr, output_scores, output_logits)
+
+    def _generate_output(self, sequences: torch.Tensor, tr: GenerateTrace, output_scores: bool,
+                         output_logits: bool) -> MedusaGenerateOutput:
+        """Read back what the scoring kernel recorded during the last loop (``wm_last_scores``)."""
+        lib = _lib.load()
+        n_tok, n_rows = C.c_int32(0), C.c_int32(0)
+        cap = max(1, len(tr.sequences))
+        lp = torch.empty(cap, dtype=torch.float32)
+        want_rows = output_scores or output_logits
+        V = self.config.vocab_size
+        rows = torch.empty((max(1, tr.iterations) if want_rows else 1), V, dtype=torch.float32)
+        _check(lib, self._handle,
+               lib.wm_last_scores(self._handle, C.cast(lp.data_ptr(), C.POINTER(C.c_float)), cap, C.byref(n_tok),
+                                  C.cast(rows.data_ptr(), C.POINTER(C.c_float)) if want_rows else None,
+                                  rows.shape[0], C.byref(n_rows) if want_rows else None), "wm_last_scores")
+        if n_tok.value < tr.n_new_tokens:
+            raise EngineError(f"wm_last_scores returned {n_tok.value} log-probabilities for {tr.n_new_tokens} tokens")
+        token_logprobs = lp[: tr.n_new_tokens]
+        avg = float(token_logprobs.double().mean())
+        rows_t = None
+        if want_rows:
+            if n_rows.value != tr.iterations:
+                raise EngineError(f"wm_last_scores returned {n_rows.value} rows for {tr.iterations} iterations")
+            dev = rows[: tr.iterations].to(self._device)
+            rows_t = tuple(dev[i : i + 1] for i in range(tr.iterations))
+        return MedusaGenerateOutput(sequences=sequences, scores=rows_t if output_scores else None,
+                                    logits=rows_t if output_logits else None,
+                                    token_logprobs=token_logprobs[None].to(self._device), avg_logprob=avg,
+                                    accept_lengths=list(tr.accept_lengths))
 
     # ------------------------------------------------------------------ forward (reference model.py:1223-1347)
     def forward(self, input_features: Optional[torch.Tensor] = None, attention_mask=None,
