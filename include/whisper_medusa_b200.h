@@ -7,6 +7,7 @@
  *     :265-291   from_pretrained(path)          -> wm_create + wm_tensor_info/wm_load_weights
  *     :1419-1449 generate(input_features, ...)  -> wm_encode_mel / wm_encode_pcm + wm_generate
  *     :1223-1347 forward(...).logits            -> wm_last_logits (parity tap)
+ *     medusa_utils.py:424-588 candidates and typical acceptance -> wm_last_accept (parity tap)
  * Each entry point below names the reference lines it replaces.  The Python host
  * (whisper_medusa_b200/model.py) binds exactly these symbols with ctypes; INTEGRATION.md shows
  * the stub a reference maintainer would add.
@@ -159,6 +160,15 @@ int wm_get_encoder_out(wm_handle* h, float* out /* [max_source_positions][d_mode
  * verify row ([n_tree][V], rows = tree nodes level by level, the order of the reference's tree_indices; n_tree = K+1
  * for a chain, up to 16 for a branching medusa_choices tree). */
 int wm_last_logits(wm_handle* h, int32_t which, float* out);
+/* What the accept step of the last iteration of the last wm_generate compared (medusa_utils.py:424-458 candidates,
+ * :526-588 evaluate_posterior), WM_MAX_T (16) entries each, indexed by verify row / tree node (chain: node n = position n):
+ * cand = token of every node; row_argmax = argmax of every processed verify row; row_pc[n] (n >= 1) = probability of
+ * node n's token in the temperature-scaled posterior of its parent row; row_thr[r] = min(posterior_threshold,
+ * posterior_alpha * exp(-entropy)) of row r; *path_node = tree only: the node at depth accept of the best path.
+ * row_pc / row_thr are not written at temperature 0; entries beyond the rows the step used are stale.  Any output may
+ * be NULL.  WM_ERR_STATE unless the last call that ran the decode loop was a completed wm_generate (wm_forward also
+ * rewrites the loop state). */
+int wm_last_accept(wm_handle* h, int32_t* cand, int32_t* row_argmax, float* row_pc, float* row_thr, int32_t* path_node);
 /* Device time (CUDA events on the handle's stream) of the last call: 0 = mel, 1 = encoder
  * (+cross K/V), 2 = decode loop.  Milliseconds. */
 double wm_last_ms(wm_handle* h, int32_t what);

@@ -62,6 +62,8 @@ SYMBOLS = {
     "wm_get_mel": (C.c_int, [C.c_void_p, _P(C.c_float)]),
     "wm_get_encoder_out": (C.c_int, [C.c_void_p, _P(C.c_float)]),
     "wm_last_logits": (C.c_int, [C.c_void_p, C.c_int32, _P(C.c_float)]),
+    "wm_last_accept": (C.c_int, [C.c_void_p, _P(C.c_int32), _P(C.c_int32), _P(C.c_float), _P(C.c_float),
+                                 _P(C.c_int32)]),
     "wm_last_ms": (C.c_double, [C.c_void_p, C.c_int32]),
     "wm_last_launches": (C.c_int64, [C.c_void_p, C.c_int32]),
     "wm_decode_cluster": (C.c_int, [C.c_void_p]),

@@ -107,6 +107,7 @@ struct wm_handle {
   float* score_lp = nullptr;    // [WM_MAX_POS + 32] log-probability per position
   float* score_rows = nullptr;  // [max_target_positions][V] scores rows
   int last_score_bits = 0, last_prompt = 0, last_L = 0, last_iters = 0;   // what the last wm_generate scored
+  int st_from_generate = 0;   // 1 while `st` holds the last iteration of a completed wm_generate (wm_last_accept)
 };
 
 static_assert(offsetof(DecState, tree_attn) == 60, "the 16 header words of DecState (L .. tree_attn) are patched as one 64-byte copy");
@@ -843,6 +844,7 @@ extern "C" int wm_generate(wm_handle* h, const int32_t* prompt, int32_t n_prompt
   cudaStream_t s = h->stream;
   h->launches[2] = 0;
   h->last_score_bits = 0;
+  h->st_from_generate = 0;
 
   // EOS exponential-decay penalty table (HF logits_process.py:1742-1772): indexed by cur_len
   if (gp->penalty_start != h->last_pen_start || gp->penalty_factor != h->last_pen_factor || n_prompt != h->last_pen_prompt) {
@@ -964,6 +966,22 @@ extern "C" int wm_generate(wm_handle* h, const int32_t* prompt, int32_t n_prompt
     CK(cudaMemcpy(accept_lens, reinterpret_cast<const char*>(h->st) + offsetof(DecState, accept_hist),
                   (size_t)iters * sizeof(int), cudaMemcpyDeviceToHost));
   h->last_score_bits = score_bits; h->last_prompt = n_prompt; h->last_L = L; h->last_iters = iters;
+  h->st_from_generate = 1;
+  return WM_OK;
+}
+
+extern "C" int wm_last_accept(wm_handle* h, int32_t* cand, int32_t* row_argmax, float* row_pc, float* row_thr,
+                              int32_t* path_node) {
+  if (!h) return WM_ERR_INVALID;
+  if (!h->st_from_generate) return fail(h, WM_ERR_STATE, "the loop state is not that of a completed wm_generate");
+  CK(cudaSetDevice(h->device));
+  const char* st = reinterpret_cast<const char*>(h->st);
+  if (cand) CK(cudaMemcpy(cand, st + offsetof(DecState, cand), WM_MAX_T * sizeof(int), cudaMemcpyDeviceToHost));
+  if (row_argmax)
+    CK(cudaMemcpy(row_argmax, st + offsetof(DecState, row_argmax), WM_MAX_T * sizeof(int), cudaMemcpyDeviceToHost));
+  if (row_pc) CK(cudaMemcpy(row_pc, st + offsetof(DecState, row_pc), WM_MAX_T * sizeof(float), cudaMemcpyDeviceToHost));
+  if (row_thr) CK(cudaMemcpy(row_thr, st + offsetof(DecState, row_thr), WM_MAX_T * sizeof(float), cudaMemcpyDeviceToHost));
+  if (path_node) CK(cudaMemcpy(path_node, st + offsetof(DecState, path_node), sizeof(int), cudaMemcpyDeviceToHost));
   return WM_OK;
 }
 
@@ -1003,6 +1021,7 @@ extern "C" int wm_forward(wm_handle* h, const int32_t* ids, int32_t n_ids, float
   cudaStream_t s = h->stream;
   const int K = h->cfg.medusa_num_heads;
   const size_t V = (size_t)h->cfg.vocab_size;
+  h->st_from_generate = 0;   // the loop state is rewritten below
   for (int t = 1; t <= n_ids; ++t) {
     DecState& hs = *h->h_init;
     memset(&hs, 0, sizeof hs);

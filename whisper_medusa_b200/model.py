@@ -627,6 +627,7 @@ class WhisperMedusaModel:
         _check(lib, self._handle, lib.wm_set_option(self._handle, b"scores", score_bits), "wm_set_option(scores)")
         tr = self._run_loop(prompt, gp)
         self.last_trace = tr
+        self._last_medusa_temperature = float(gp.temperature)
         out = self._strip(tr.sequences, len(prompt), int(gp.pad_token_id), int(gp.eos_token_id))
         sequences = torch.tensor([out], dtype=torch.long, device=self._device)
         if not as_dict:
@@ -723,6 +724,36 @@ class WhisperMedusaModel:
         _check(lib, self._handle, lib.wm_last_logits(self._handle, which, C.cast(out.data_ptr(), C.POINTER(C.c_float))),
                "wm_last_logits")
         return out
+
+    def last_accept(self) -> Dict[str, Optional[Union[torch.Tensor, int]]]:
+        """What the accept step of the last ``generate`` iteration compared (``wm_last_accept``), one entry per verify row
+        / tree node (``n_tree`` = K+1 for a chain): ``cand`` the node tokens, ``row_argmax`` the argmax of every processed
+        verify row, ``row_pc[n]`` (n >= 1) the probability of node n's token under its parent row's posterior,
+        ``row_thr[r]`` the acceptance threshold ``min(posterior_threshold, posterior_alpha * exp(-entropy))`` of row r,
+        ``path_node`` (trees only, else None) the node at depth ``accept`` of the best path.  ``row_pc`` and ``row_thr``
+        are None at ``medusa_temperature=0`` (exact-match acceptance computes neither); entries of rows that have no
+        child (chain: ``row_thr[K]``; ``row_pc[0]``) are not part of the decision."""
+        self._require_engine()
+        nt = self.config.medusa_num_heads + 1
+        tree = any(int(c) != 1 for c in self.config.medusa_choices)
+        if tree:
+            nt, level = 0, 1
+            for c in self.config.medusa_choices:
+                level *= int(c)
+                nt += level
+        cand = torch.empty(16, dtype=torch.int32)
+        arg = torch.empty(16, dtype=torch.int32)
+        pc = torch.empty(16, dtype=torch.float32)
+        thr = torch.empty(16, dtype=torch.float32)
+        node = C.c_int32(0)
+        lib = _lib.load()
+        _check(lib, self._handle,
+               lib.wm_last_accept(self._handle, C.cast(cand.data_ptr(), C.POINTER(C.c_int32)),
+                                  C.cast(arg.data_ptr(), C.POINTER(C.c_int32)), C.cast(pc.data_ptr(), C.POINTER(C.c_float)),
+                                  C.cast(thr.data_ptr(), C.POINTER(C.c_float)), C.byref(node)), "wm_last_accept")
+        typical = getattr(self, "_last_medusa_temperature", 1.0) != 0.0
+        return {"cand": cand[:nt], "row_argmax": arg[:nt], "row_pc": pc[:nt] if typical else None,
+                "row_thr": thr[:nt] if typical else None, "path_node": int(node.value) if tree else None}
 
     def encoder_output(self) -> torch.Tensor:
         self._require_engine()
