@@ -146,6 +146,14 @@ int wm_generate(wm_handle* h, const int32_t* prompt, int32_t n_prompt, const wm_
  * Either output may be NULL.  WM_ERR_STATE if the last wm_generate did not record what is asked for. */
 int wm_last_scores(wm_handle* h, float* token_logprobs, int32_t cap, int32_t* n_tokens, float* rows, int32_t cap_rows,
                    int32_t* n_rows);
+/* No-speech probability of the last wm_generate (option "no_speech_row" = the prompt index of the SOT row, set before
+ * the call; HF WhisperNoSpeechDetection).  The loop keeps that row's final-LayerNorm hidden state, and one launch after
+ * the loop (two for the base_head type, whose base row goes through head 0 first) computes the row's raw base-head
+ * logits -- forward(decoder_input_ids=[SOT], disable_medusa=True) -- and their log-sum-exp.
+ * prob (may be NULL) = exp(logit[token] - lse), token = no_timestamps_token_id - 1 for HF's choice; row_logits
+ * (vocab_size floats, may be NULL) = the raw row.  WM_ERR_STATE if the last wm_generate computed no row, or its loop
+ * did not capture the SOT row (the capture buffer is set to NaN before every such loop).  wm_forward never captures. */
+int wm_last_no_speech(wm_handle* h, int32_t token, float* prob, float* row_logits);
 
 /* ---- teacher-forced forward (model.py:1223-1347 `forward(...).logits`, shape [K+1, 1, T, V]) -------------- */
 /* ids: 1..16 decoder_input_ids; out (host, capacity (K+1) * n_ids * vocab_size floats) receives the raw logits of
@@ -191,7 +199,10 @@ void* wm_weights_device_ptr(wm_handle* h);
  * shapes); "enc_attn" 1 = wgmma/TMA encoder attention (default), 0 = mma.sync flash attention (cross-check);
  * "enc_pdl" 1 = encoder kernels under programmatic dependent launch (default), 0 = plain stream-ordered launches;
  * "profile" 1 = record the stage timeline below; "scores" = what wm_generate records for wm_last_scores: bit 0 the
- * per-token log-probabilities, bit 1 the scores rows (0, the default: nothing, and no extra launch). */
+ * per-token log-probabilities, bit 1 the scores rows (0, the default: nothing, and no extra launch);
+ * "no_speech_row" = prompt index of the SOT row whose no-speech probability wm_generate computes (wm_last_no_speech;
+ * -1, the default: off, and no extra launch).  wm_generate returns WM_ERR_UNSUPPORTED if that row falls in a prefill
+ * chunk of a long prompt (the SOT row must be among the last ((n_prompt - 1) % 16) + 1 rows). */
 int wm_set_option(wm_handle* h, const char* key, int32_t value);
 /* Host logic, no GPU needed: the tile {rows, columns, ring stages} the wgmma encoder GEMM runs an M x N x K product
  * with on a GPU of n_sm SMs (0: 132) -- the shape with the fewest operand bytes on the busiest SM (DESIGN.md section 4).

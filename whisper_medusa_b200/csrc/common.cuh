@@ -281,6 +281,10 @@ struct alignas(16) DecModel {   // (copied to shared memory in 16-byte pieces by
   DecState* st;
   unsigned int* bar;  // grid-barrier words for the persistent kernel
   unsigned long long* prof;  // optional stage timeline [2 CTAs][n_instr][16] (ns, and flags), null = off
+  // no-speech capture (option "no_speech_row"): the final LayerNorm stores row ns_row of the first real iteration's
+  // sweep A (row index within that pass's tile, prefill chunks excluded) into ns_hidden [d]; -1 = off
+  float* ns_hidden;
+  int ns_row;
 };
 
 }  // namespace wm

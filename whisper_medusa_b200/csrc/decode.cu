@@ -747,7 +747,17 @@ __global__ void __launch_bounds__(256) relayout_cross_kv_kernel(const __half* __
 //   sweep A: the last row is also the "carry" (hidden state of the newest cached token, the
 //            input of the Medusa heads).  sweep B + block type: base logits read the hidden
 //            states directly (reference model.py:1287).
+//   no-speech capture: row m->ns_row of the first real iteration's sweep A (n_iter == 0, not a
+//            prefill launch) is also stored into m->ns_hidden (read after the loop by no_speech.cu).
 // -----------------------------------------------------------------------------------------
+// no-speech capture (out of line: the rare branch adds no registers to the stage): warp 0 copies back the row it has
+// just stored, each lane only the elements it stored itself
+__device__ __noinline__ void ns_capture(const DecModel* m, int t) {
+  if (ldcg_i(&m->st->n_iter) != 0 || ldcg_i(&m->st->prefill)) return;
+  const float4* src = reinterpret_cast<const float4*>(m->hidden + (size_t)t * m->d);
+  float4* dst = reinterpret_cast<float4*>(m->ns_hidden);
+  for (int i = threadIdx.x & 31; i < (m->d >> 2); i += 32) dst[i] = __ldcg(src + i);
+}
 __device__ __forceinline__ void stage_final_ln(const DecModel* m, int mode, int cta, int ncta, const PassGeom* gopt) {
   const PassGeom g = gopt ? *gopt : pass_geom(m, mode);
   const int d = m->d;
@@ -790,6 +800,7 @@ __device__ __forceinline__ void stage_final_ln(const DecModel* m, int mode, int 
         if (mode == MODE_A && t == g.T - 1) reinterpret_cast<float4*>(m->carry)[i * 32 + lane] = y;
         if (mode == MODE_B && m->has_block) reinterpret_cast<float4*>(m->head_h + (size_t)t * d)[i * 32 + lane] = y;
       }
+    if (mode == MODE_A && t == m->ns_row) ns_capture(m, t);
   }
 }
 // block type: the extra layer consumes the LayerNorm'ed hidden states (reference model.py:1374-1376)

@@ -108,6 +108,13 @@ struct wm_handle {
   float* score_rows = nullptr;  // [max_target_positions][V] scores rows
   int last_score_bits = 0, last_prompt = 0, last_L = 0, last_iters = 0;   // what the last wm_generate scored
   int st_from_generate = 0;   // 1 while `st` holds the last iteration of a completed wm_generate (wm_last_accept)
+  // no-speech row (option "no_speech_row": index in the prompt of the SOT row, -1 = off); buffers allocated on first use
+  int ns_prompt_row = -1;
+  float* ns_head = nullptr;     // [d] base_head type: the row after head 0
+  float* ns_logits = nullptr;   // [V] raw base-head logits of the row
+  float* ns_part = nullptr;     // [WM_NS_NSEG][2] segment partials, then [1] log-sum-exp
+  unsigned int* ns_count = nullptr;
+  int last_ns = 0;              // 1: the last wm_generate computed the row
 };
 
 static_assert(offsetof(DecState, tree_attn) == 60, "the 16 header words of DecState (L .. tree_attn) are patched as one 64-byte copy");
@@ -338,6 +345,7 @@ extern "C" int wm_create(const wm_config* cfg, int device, wm_handle** out) {
   CK(dalloc(&h->bar, 8));
   CK(dalloc(&h->dm, 1));
   m.st = h->st; m.tok_mask = h->tok_mask; m.pen_tab = h->pen_tab; m.bar = h->bar;
+  m.ns_row = -1;
   CK(cudaMallocHost((void**)&h->h_state, 64 * sizeof(int)));
   CK(cudaMallocHost((void**)&h->h_stage, (size_t)kSamples * sizeof(float)));
   CK(cudaMallocHost((void**)&h->h_init, sizeof(DecState)));
@@ -389,6 +397,7 @@ extern "C" int wm_destroy(wm_handle* h) {
   F(h->hm.x); F(h->hm.xg); F(h->hm.q); F(h->hm.attn); F(h->hm.ffn_h); F(h->hm.hidden); F(h->hm.head_h); F(h->hm.carry); F(h->hm.cross_part); F(h->hm.cross_cnt); F(h->hm.sel_part); F(h->hm.gemm_part); F(h->hm.gemm_cnt);
   F(h->hm.topk_part); F(h->tree); F(h->hm.logits_a); F(h->hm.logits_b); F(h->st); F(h->tok_mask); F(h->pen_tab); F(h->bar); F(h->prof); F(h->chunk_tab); F(h->chunk_off); F(h->stage_tab); F(h->ln_fold); F(h->dm);
   F(h->score_state); F(h->score_part); F(h->score_lp); F(h->score_rows);
+  F(h->hm.ns_hidden); F(h->ns_head); F(h->ns_logits); F(h->ns_part); F(h->ns_count);
   if (h->wowned) F(h->wdev);
   for (auto& kv : h->resamplers) { F(kv.second.taps); F(kv.second.sup); }
   if (h->h_state) cudaFreeHost(h->h_state);
@@ -830,6 +839,16 @@ static int64_t enqueue_iteration(wm_handle* h, int mode, int rows, int last_phas
   return n;
 }
 
+// The final-LayerNorm row the decode loop copies into ns_hidden (DecModel::ns_row, -1 = none): changes the device
+// copy in stream order when it differs.
+static int set_ns_row(wm_handle* h, int row) {
+  if (row == h->hm.ns_row) return WM_OK;
+  h->hm.ns_row = row;
+  CK(cudaMemcpyAsync(reinterpret_cast<char*>(h->dm) + offsetof(DecModel, ns_row), &h->hm.ns_row, sizeof(int),
+                     cudaMemcpyHostToDevice, h->stream));
+  return WM_OK;
+}
+
 extern "C" int wm_generate(wm_handle* h, const int32_t* prompt, int32_t n_prompt, const wm_gen_params* gp,
                            int32_t* out_ids, int32_t* n_out, int32_t* accept_lens, int32_t* n_iter) {
   if (!h || !prompt || !gp || !out_ids || !n_out) return WM_ERR_INVALID;
@@ -840,11 +859,24 @@ extern "C" int wm_generate(wm_handle* h, const int32_t* prompt, int32_t n_prompt
   if (gp->temperature < 0.f) return fail(h, WM_ERR_INVALID, "temperature must be >= 0");
   for (int i = 0; i < n_prompt; ++i)
     if (prompt[i] < 0 || prompt[i] >= h->cfg.vocab_size) return fail(h, WM_ERR_INVALID, "prompt id out of range");
+  // the no-speech row must be computed by the first real iteration: not in a prefill chunk (the first
+  // n_prompt - n_tail rows, n_tail below)
+  const int ns_tail0 = (n_prompt - 1) / WM_MAX_T * WM_MAX_T;   // = n_prompt - n_tail
+  if (h->ns_prompt_row >= n_prompt) return fail(h, WM_ERR_INVALID, "no_speech_row is beyond the prompt");
+  if (h->ns_prompt_row >= 0 && h->ns_prompt_row < ns_tail0)
+    return fail(h, WM_ERR_UNSUPPORTED, "no_speech_row falls in a prefill chunk of the prompt (not in its last rows)");
   CK(cudaSetDevice(h->device));
   cudaStream_t s = h->stream;
   h->launches[2] = 0;
   h->last_score_bits = 0;
   h->st_from_generate = 0;
+  h->last_ns = 0;
+  {
+    const int r = set_ns_row(h, h->ns_prompt_row >= 0 ? h->ns_prompt_row - ns_tail0 : -1);
+    if (r != WM_OK) return r;
+    // a row the loop fails to capture stays NaN, and so do its logits: wm_last_no_speech then refuses them
+    if (h->hm.ns_row >= 0) CK(cudaMemsetAsync(h->hm.ns_hidden, 0xFF, (size_t)h->hm.d * sizeof(float), s));
+  }
 
   // EOS exponential-decay penalty table (HF logits_process.py:1742-1772): indexed by cur_len
   if (gp->penalty_start != h->last_pen_start || gp->penalty_factor != h->last_pen_factor || n_prompt != h->last_pen_prompt) {
@@ -908,6 +940,7 @@ extern "C" int wm_generate(wm_handle* h, const int32_t* prompt, int32_t n_prompt
       n_tail = n_prompt - pos;
     }
   }
+
   if (h->decode_mode == 0) {
     // capture the graphs of this call before the timed loop ({phase, rows}: the rows only key the sweep-A graphs; there
     // is one tail and one verify graph, and the verify rows come from n_tree)
@@ -944,6 +977,15 @@ extern "C" int wm_generate(wm_handle* h, const int32_t* prompt, int32_t n_prompt
     done = h->h_state[2];
     iters = h->h_state[3];
   }
+  if (h->hm.ns_row >= 0) {   // the base-head row of the captured SOT hidden state (no_speech.cu)
+    NoSpeechArgs na;
+    na.hidden = h->hm.ns_hidden;
+    na.head_w = h->hm.has_block ? nullptr : h->hm.heads_w;
+    na.head_b = h->hm.heads_b;
+    na.head_out = h->ns_head; na.embed = h->hm.embed; na.d = h->hm.d; na.V = h->hm.V;
+    na.logits = h->ns_logits; na.part = h->ns_part; na.lse = h->ns_part + 2 * WM_NS_NSEG; na.count = h->ns_count;
+    CK(dec_launch_no_speech(na, h->n_cta, s, &h->launches[2]));
+  }
   CK(cudaEventRecord(h->ev[4], s));
   CK(cudaStreamSynchronize(s));
   float tms = 0;
@@ -967,6 +1009,22 @@ extern "C" int wm_generate(wm_handle* h, const int32_t* prompt, int32_t n_prompt
                   (size_t)iters * sizeof(int), cudaMemcpyDeviceToHost));
   h->last_score_bits = score_bits; h->last_prompt = n_prompt; h->last_L = L; h->last_iters = iters;
   h->st_from_generate = 1;
+  h->last_ns = h->hm.ns_row >= 0;
+  return WM_OK;
+}
+
+extern "C" int wm_last_no_speech(wm_handle* h, int32_t token, float* prob, float* row_logits) {
+  if (!h) return WM_ERR_INVALID;
+  if (!h->last_ns) return fail(h, WM_ERR_STATE, "the last wm_generate computed no no-speech row (option \"no_speech_row\")");
+  if (token < 0 || token >= h->cfg.vocab_size) return fail(h, WM_ERR_INVALID, "token out of range");
+  CK(cudaSetDevice(h->device));
+  float v[2];
+  CK(cudaMemcpy(&v[0], h->ns_logits + token, sizeof(float), cudaMemcpyDeviceToHost));
+  CK(cudaMemcpy(&v[1], h->ns_part + 2 * WM_NS_NSEG, sizeof(float), cudaMemcpyDeviceToHost));
+  // (ns_hidden is NaN before every loop that captures: a finite log-sum-exp means the loop stored the row)
+  if (!std::isfinite(v[1])) return fail(h, WM_ERR_STATE, "the last wm_generate did not capture the SOT row");
+  if (prob) *prob = std::exp(v[0] - v[1]);
+  if (row_logits) CK(cudaMemcpy(row_logits, h->ns_logits, (size_t)h->cfg.vocab_size * sizeof(float), cudaMemcpyDeviceToHost));
   return WM_OK;
 }
 
@@ -1022,6 +1080,10 @@ extern "C" int wm_forward(wm_handle* h, const int32_t* ids, int32_t n_ids, float
   const int K = h->cfg.medusa_num_heads;
   const size_t V = (size_t)h->cfg.vocab_size;
   h->st_from_generate = 0;   // the loop state is rewritten below
+  {
+    const int r = set_ns_row(h, -1);   // (the passes below must not overwrite the last wm_generate's captured row)
+    if (r != WM_OK) return r;
+  }
   for (int t = 1; t <= n_ids; ++t) {
     DecState& hs = *h->h_init;
     memset(&hs, 0, sizeof hs);
@@ -1131,6 +1193,25 @@ extern "C" int wm_set_option(wm_handle* h, const char* key, int32_t value) {
     if ((value & 2) && !h->score_rows)
       CK(dalloc(&h->score_rows, (size_t)h->cfg.max_target_positions * h->cfg.vocab_size));
     h->score_bits = value;
+    return WM_OK;
+  }
+  if (k == "no_speech_row") {
+    // index in the prompt of the SOT row whose base-head logits the next wm_generate computes (wm_last_no_speech);
+    // -1 (the default): off, and the loop launches exactly what it launches without it
+    if (value < -1) return fail(h, WM_ERR_INVALID, "no_speech_row must be -1 (off) or a prompt index");
+    if (h->device < 0) return fail(h, WM_ERR_STATE, "layout-only handle");
+    CK(cudaSetDevice(h->device));
+    if (value >= 0 && !h->ns_logits) {
+      CK(cudaStreamSynchronize(h->stream));   // (the device model description is rewritten below)
+      CK(dalloc(&h->hm.ns_hidden, (size_t)h->hm.d));
+      CK(dalloc(&h->ns_head, (size_t)h->hm.d));
+      CK(dalloc(&h->ns_logits, (size_t)h->cfg.vocab_size));
+      CK(dalloc(&h->ns_part, (size_t)2 * WM_NS_NSEG + 1));
+      CK(dalloc(&h->ns_count, 1));
+      CK(cudaMemset(h->ns_count, 0, sizeof(unsigned int)));
+      CK(cudaMemcpy(h->dm, &h->hm, sizeof(DecModel), cudaMemcpyHostToDevice));
+    }
+    h->ns_prompt_row = value;
     return WM_OK;
   }
   if (k == "enc_attn") {

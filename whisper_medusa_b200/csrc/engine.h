@@ -69,6 +69,26 @@ struct ScoreArgs {
 int dec_score_grid(int n_cta, int K);
 cudaError_t dec_launch_scores(const ScoreArgs& a, int grid, cudaStream_t s);
 
+// ---- no_speech.cu ----
+#define WM_NS_NSEG 512         // vocabulary segments of the no-speech row (fixed: the fold order does not depend on the grid)
+#define WM_NS_THREADS 512
+// The base-head logits of the captured SOT row and their log-sum-exp; launched once after the loop when capture is on.
+struct NoSpeechArgs {
+  const float* hidden;     // [d] final-LayerNorm row captured by the loop (DecModel::ns_hidden)
+  const __half* head_w;    // base_head type: head 0 [d, d] (the row goes through it first); null for medusa_block
+  const float* head_b;     // [d]
+  float* head_out;         // [d] base_head type: hidden + SiLU(head_w . hidden + head_b)
+  const __half* embed;     // [V, d] proj_out (tied)
+  int d, V;
+  float* logits;           // [V] raw logits
+  float* part;             // [WM_NS_NSEG]{max, sum of exp(v - max)}
+  float* lse;              // [1] log-sum-exp of the row
+  unsigned int* count;     // arrival counter (zero between launches)
+};
+// grid: CTAs of each launch (<= decode_ctas); enqueues 2 kernels for the base_head type (head 0, then the vocabulary
+// product), 1 for medusa_block, and adds them to *n_launch
+cudaError_t dec_launch_no_speech(const NoSpeechArgs& a, int grid, cudaStream_t s, int64_t* n_launch);
+
 // ---- mel.cu ----
 // pcm: device f32 [480000] (already zero padded). Outputs: mel_f32 [80][3000], xT fp16 [rows>=3000+?][80]
 // time-major with one leading zero row (conv padding); gmax_bits: device scratch (1 int).

@@ -16,7 +16,10 @@ scores (`metrics.py` restates jiwer 3.0.3, see there).  Differences, all on the 
   calls `generate(input_features)` exactly as the reference does (`eval_whisper_medusa.py:46-65`);
 * `--chunk-length-s S` (S > 0, at most 30) reads each file at its native rate and transcribes it with
   `model.transcribe(pcm, sampling_rate=sr, chunk_length_s=S)`: recordings of any length, resampled on the GPU
-  (the reference accepts at most 30 s).  The default 0 keeps the path above.
+  (the reference accepts at most 30 s).  The default 0 keeps the path above;
+* `--no-speech-threshold P --logprob-threshold L`: HF's no-speech rule.  Chunked mode passes both to `transcribe`
+  (silent windows add no text); otherwise each clip's `generate` dict output is tested with the same rule
+  (`longform.skip_window`) and a silent clip's hypothesis is empty.
 """
 from __future__ import annotations
 
@@ -100,12 +103,16 @@ def evaluate_rows(rows: Iterable[Dict], transcribe: Callable[[np.ndarray, str], 
 
 def evaluate_model(model_name: str, data_path: str, out_file_path: str, language: str = "en",
                    regulation_start: float = 140, regulation_factor: float = 1.0, frontend: str = "engine",
-                   device: str = "cuda:0", chunk_length_s: float = 0.0):
+                   device: str = "cuda:0", chunk_length_s: float = 0.0, no_speech_threshold: Optional[float] = None,
+                   logprob_threshold: Optional[float] = None):
     import pandas as pd
     import torch
     from transformers import WhisperProcessor
 
     from . import WhisperMedusaModel
+    from .longform import no_speech_rule, skip_window
+
+    rule = no_speech_rule(no_speech_threshold, logprob_threshold)
 
     data = pd.read_csv(data_path).fillna("")
     processor = WhisperProcessor.from_pretrained(model_name)
@@ -116,12 +123,19 @@ def evaluate_model(model_name: str, data_path: str, out_file_path: str, language
         if chunk_length_s > 0:
             x, sr = pcm
             out = model.transcribe(x, sampling_rate=sr, chunk_length_s=chunk_length_s, language=lang,
-                                   exponential_decay_length_penalty=penalty)
-        elif frontend == "hf":
+                                   exponential_decay_length_penalty=penalty, no_speech_threshold=no_speech_threshold,
+                                   logprob_threshold=logprob_threshold)
+            return processor.decode(out[0], skip_special_tokens=True)
+        ns = dict(return_dict_in_generate=True, output_no_speech_prob=True) if rule else {}
+        if frontend == "hf":
             feats = processor(pcm, return_tensors="pt", sampling_rate=SAMPLING_RATE).input_features
-            out = model.generate(feats, language=lang, exponential_decay_length_penalty=penalty)
+            out = model.generate(feats, language=lang, exponential_decay_length_penalty=penalty, **ns)
         else:
-            out = model.generate_from_pcm(pcm, language=lang, exponential_decay_length_penalty=penalty)
+            out = model.generate_from_pcm(pcm, language=lang, exponential_decay_length_penalty=penalty, **ns)
+        if rule:
+            if skip_window(out.no_speech_prob, out.avg_logprob, no_speech_threshold, logprob_threshold):
+                return ""
+            out = out.sequences
         return processor.decode(out[0], skip_special_tokens=True)
 
     with torch.no_grad():
@@ -149,10 +163,15 @@ def main(argv: Optional[Sequence[str]] = None):
     ap.add_argument("--device", type=str, default="cuda:0")
     ap.add_argument("--chunk-length-s", type=float, default=0.0,
                     help="> 0: long-form transcription in windows of this many seconds (at most 30) at the file's own rate")
+    ap.add_argument("--no-speech-threshold", type=float, default=None,
+                    help="skip a window / clip whose <|nospeech|> probability is above this (needs --logprob-threshold)")
+    ap.add_argument("--logprob-threshold", type=float, default=None,
+                    help="... and whose average token log-probability is below this")
     args = ap.parse_args(argv)
     logging.basicConfig(format="%(asctime)s - %(name)s - %(levelname)s - %(message)s", level=logging.INFO)
     evaluate_model(args.model_name, args.data_path, args.out_file_path, args.language, args.regulation_start,
-                   args.regulation_factor, args.frontend, args.device, args.chunk_length_s)
+                   args.regulation_factor, args.frontend, args.device, args.chunk_length_s, args.no_speech_threshold,
+                   args.logprob_threshold)
 
 
 if __name__ == "__main__":

@@ -10,6 +10,9 @@ timestamps, so that a recording of any length transcribes as that pipeline would
   token timestamps: consecutive windows are aligned where their ids agree best, the left window's ids are kept up to
   the middle of the overlap and the right window's from there on.
 
+With ``no_speech_threshold`` and ``logprob_threshold``, a window is skipped by HF's no-speech rule (``skip_window``) and
+contributes no ids to the merge.
+
 The CPU tests pin both to the installed transformers; the package does not import it.
 """
 from __future__ import annotations
@@ -106,6 +109,34 @@ def text_ids(ids: Sequence[int], eos_token_id: int) -> List[int]:
     return [int(t) for t in ids if int(t) < eos_token_id]
 
 
+def no_speech_rule(no_speech_threshold, logprob_threshold) -> bool:
+    """Check the no-speech arguments of ``transcribe``; True when windows are to be tested for silence.
+
+    HF's rule needs both thresholds: ``no_speech_threshold`` alone raises ``ValueError`` (HF itself fails comparing
+    with ``None`` there).  ``logprob_threshold`` alone means temperature fallback, which greedy-only Medusa decoding
+    cannot do: ``NotImplementedError``.  Both must be finite numbers."""
+    if no_speech_threshold is None and logprob_threshold is None:
+        return False
+    if logprob_threshold is None:
+        raise ValueError("no_speech_threshold needs logprob_threshold: a window is skipped when its no-speech "
+                         "probability is above the first and its average log-probability below the second")
+    if no_speech_threshold is None:
+        raise NotImplementedError("logprob_threshold without no_speech_threshold asks for temperature fallback, which "
+                                  "is not supported with medusa (greedy search only)")
+    for name, v in (("no_speech_threshold", no_speech_threshold), ("logprob_threshold", logprob_threshold)):
+        if isinstance(v, bool) or not isinstance(v, (int, float, np.floating, np.integer)) or not math.isfinite(float(v)):
+            raise ValueError(f"{name} must be a finite float, got {v!r}")
+    return True
+
+
+def skip_window(no_speech_prob: float, avg_logprob: float, no_speech_threshold: float,
+                logprob_threshold: float) -> bool:
+    """HF ``WhisperGenerationMixin._need_fallback``'s ``should_skip``: the window is silent when the probability of
+    ``<|nospeech|>`` at the start-of-transcript position is above ``no_speech_threshold`` and the average log-probability
+    of its tokens is below ``logprob_threshold`` (both strict)."""
+    return avg_logprob < logprob_threshold and no_speech_prob > no_speech_threshold
+
+
 def resampled_length(n: int, orig_hz: int, new_hz: int) -> int:
     """``ceil(n * new / orig)`` with the rates divided by their gcd (torchaudio's output length)."""
     g = math.gcd(int(orig_hz), int(new_hz))
@@ -116,11 +147,21 @@ def resampled_length(n: int, orig_hz: int, new_hz: int) -> int:
 class WindowResult:
     """One window of a long-form transcription (``WhisperMedusaModel.last_windows``)."""
 
-    def __init__(self, window: Window, ids: List[int], trace):
+    def __init__(self, window: Window, ids: List[int], trace, no_speech_prob: Optional[float] = None,
+                 avg_logprob: Optional[float] = None, skipped: Optional[bool] = None):
         self.start, self.end = window.start, window.end
         self.stride_left, self.stride_right = window.stride_left, window.stride_right
         self.ids = ids            # what generate() returns for the window (prompt and trailing EOS stripped)
         self.trace = trace        # its GenerateTrace
+        # no-speech rule (transcribe(no_speech_threshold=..., logprob_threshold=...); all None without it)
+        self.no_speech_prob = no_speech_prob
+        self.avg_logprob = avg_logprob
+        self.skipped = skipped    # True: the window counts as silence and adds no ids to the merge
+
+    def merge_ids(self, eos_token_id: int) -> List[int]:
+        """What the window contributes to ``merge_windows``: its text ids, or none for a skipped window (its
+        neighbours are then both kept whole: no overlap is de-duplicated across it)."""
+        return [] if self.skipped else text_ids(self.ids, eos_token_id)
 
     def __repr__(self) -> str:
         return (f"WindowResult(samples {self.start}:{self.end}, strides ({self.stride_left}, {self.stride_right}), "

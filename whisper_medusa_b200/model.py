@@ -31,8 +31,8 @@ import torch
 
 from . import _lib
 from .config import MedusaConfig, MedusaGenerationConfig
-from .longform import (MAX_WINDOW_SAMPLES, SAMPLE_RATE, Window, WindowResult, merge_windows, plan_windows,
-                       resampled_length, text_ids, window_params)
+from .longform import (MAX_WINDOW_SAMPLES, SAMPLE_RATE, Window, WindowResult, merge_windows, no_speech_rule,
+                       plan_windows, resampled_length, skip_window, window_params)
 from .weights import pack_blob
 
 N_FRAMES = 3000
@@ -116,20 +116,24 @@ class MedusaGenerateOutput:
     * ``token_logprobs``: ``FloatTensor[1, n_new_tokens]``, the log-probability (log_softmax at temperature 1 of the
       processed row) of every generated token up to and including the first EOS, under the row it was chosen from;
     * ``avg_logprob``: their mean (a float);
-    * ``accept_lengths``: the accept length of every iteration.
+    * ``accept_lengths``: the accept length of every iteration;
+    * ``no_speech_prob`` (``output_no_speech_prob=True``, else ``None``): the probability of ``<|nospeech|>``
+      (``no_timestamps_token_id - 1``) in the softmax of the raw base-head logits at the start-of-transcript position
+      (HF ``WhisperNoSpeechDetection``), computed on the GPU (``csrc/no_speech.cu``); a float.
 
     Fields are attributes and keys (``out.scores`` / ``out["scores"]``); an integer indexes the fields that are not
     ``None``, in the order above, as HF ``ModelOutput`` does."""
 
-    FIELDS = ("sequences", "scores", "logits", "token_logprobs", "avg_logprob", "accept_lengths")
+    FIELDS = ("sequences", "scores", "logits", "token_logprobs", "avg_logprob", "accept_lengths", "no_speech_prob")
 
-    def __init__(self, sequences, scores, logits, token_logprobs, avg_logprob, accept_lengths):
+    def __init__(self, sequences, scores, logits, token_logprobs, avg_logprob, accept_lengths, no_speech_prob=None):
         self.sequences = sequences
         self.scores = scores
         self.logits = logits
         self.token_logprobs = token_logprobs
         self.avg_logprob = avg_logprob
         self.accept_lengths = accept_lengths
+        self.no_speech_prob = no_speech_prob
 
     def keys(self) -> List[str]:
         return [k for k in self.FIELDS if getattr(self, k) is not None]
@@ -438,8 +442,9 @@ class WhisperMedusaModel:
                  return_dict_in_generate=None, **kwargs) -> Union[torch.Tensor, MedusaGenerateOutput]:
         """Transcribe one <= 30 s clip given its log-mel features ``[1, 80, 3000]``
         (reference ``model.py:1419-1779``); returns ``LongTensor[1, n]``, or with ``return_dict_in_generate=True`` a
-        ``MedusaGenerateOutput`` (``output_scores`` / ``output_logits`` select its ``scores`` / ``logits``; without
-        ``return_dict_in_generate`` they have no effect, as in HF and the reference)."""
+        ``MedusaGenerateOutput`` (``output_scores`` / ``output_logits`` / ``output_no_speech_prob`` select its
+        ``scores`` / ``logits`` / ``no_speech_prob``; without ``return_dict_in_generate`` they have no effect, as in HF
+        and the reference).  ``no_speech_threshold`` raises as in the reference: the skip rule is ``transcribe``'s."""
         self._require_engine()
         if input_features is None:
             raise ValueError("input_features is required")
@@ -488,7 +493,7 @@ class WhisperMedusaModel:
             raise NotImplementedError("sampling (temperature > 0 / do_sample) is not supported with medusa: greedy search only")
         known = {"exponential_decay_length_penalty", "max_length", "max_new_tokens", "max_iters", "medusa_temperature",
                  "posterior_threshold", "posterior_alpha", "num_beams", "do_sample", "use_cache", "tree_attention",
-                 "decoder_input_ids", "output_scores", "output_logits"}
+                 "decoder_input_ids", "output_scores", "output_logits", "output_no_speech_prob"}
         unknown = sorted(set(kwargs) - known)
         if unknown:
             raise NotImplementedError(f"generate() options not implemented by the H100 engine: {unknown}")
@@ -523,6 +528,7 @@ class WhisperMedusaModel:
     def transcribe(self, audio: Union[np.ndarray, torch.Tensor], sampling_rate: int = SAMPLE_RATE,
                    chunk_length_s: float = 30.0, stride_length_s: Optional[Union[float, Sequence[float]]] = None,
                    language: Optional[str] = None, task: Optional[str] = None, temperature=None,
+                   no_speech_threshold: Optional[float] = None, logprob_threshold: Optional[float] = None,
                    **generate_kwargs) -> torch.Tensor:
         """Transcribe a mono recording of any length at any integer sampling rate; returns ``LongTensor[1, n]``.
 
@@ -536,18 +542,26 @@ class WhisperMedusaModel:
         ``audio``: 1-D f32 samples as a numpy array, a CPU tensor, or a CUDA tensor on the engine's device (used in place,
         ordered after the current stream).  The recording is uploaded once and, if ``sampling_rate != 16000``, resampled
         once on the GPU.  Every window's log-mel is computed from the device-resident samples.  Per-window results go
-        to ``self.last_windows``.  An empty recording has no windows and gives ``[1, 0]``."""
+        to ``self.last_windows``.  An empty recording has no windows and gives ``[1, 0]``.
+
+        ``no_speech_threshold`` with ``logprob_threshold``: HF's no-speech rule.  A window is skipped -- it adds no ids to
+        the merge -- when the probability of ``<|nospeech|>`` at its start-of-transcript position is above
+        ``no_speech_threshold`` and the average log-probability of its tokens is below ``logprob_threshold``.  Each
+        window is still decoded in full (the rule needs its average log-probability).  ``no_speech_threshold`` alone
+        raises ``ValueError``; ``logprob_threshold`` alone (temperature fallback) ``NotImplementedError``."""
         self._require_engine()
         params = window_params(chunk_length_s, stride_length_s)
         _check_recording(audio, sampling_rate)
+        no_speech = ((float(no_speech_threshold), float(logprob_threshold))
+                     if no_speech_rule(no_speech_threshold, logprob_threshold) else None)
         self._check_unsupported(temperature, None, generate_kwargs)
         x16 = self._upload_16k(audio, sampling_rate)
         stream = torch.cuda.current_stream(self._device).cuda_stream
         results = [self._transcribe_window(x16, w, stream, language=language, task=task, temperature=temperature,
-                                           **generate_kwargs)
+                                           no_speech=no_speech, **generate_kwargs)
                    for w in plan_windows(x16.numel(), *params)]
         self.last_windows = results
-        merged = merge_windows([text_ids(r.ids, int(self.generation_config.eos_token_id)) for r in results])
+        merged = merge_windows([r.merge_ids(int(self.generation_config.eos_token_id)) for r in results])
         return torch.tensor([merged], dtype=torch.long, device=self._device)
 
     def _upload_16k(self, audio, sampling_rate) -> torch.Tensor:
@@ -583,10 +597,17 @@ class WhisperMedusaModel:
                "wm_encode_pcm_device")
 
     def _transcribe_window(self, x16: torch.Tensor, w: Window, producer_stream: int, language=None, task=None,
-                           temperature=None, **kwargs) -> WindowResult:
+                           temperature=None, no_speech: Optional[Tuple[float, float]] = None, **kwargs) -> WindowResult:
+        """One window; ``no_speech`` = (no_speech_threshold, logprob_threshold) or None (the rule off)."""
         self._encode_window(x16, w, producer_stream)
-        ids = self._decode(language, task, kwargs, temperature)[0].tolist()
-        return WindowResult(w, ids, self.last_trace)
+        if no_speech is None:
+            ids = self._decode(language, task, kwargs, temperature)[0].tolist()
+            return WindowResult(w, ids, self.last_trace)
+        out = self._decode(language, task, dict(kwargs, output_no_speech_prob=True), temperature,
+                           return_dict_in_generate=True)
+        return WindowResult(w, out.sequences[0].tolist(), self.last_trace, no_speech_prob=out.no_speech_prob,
+                            avg_logprob=out.avg_logprob,
+                            skipped=skip_window(out.no_speech_prob, out.avg_logprob, *no_speech))
 
     def _decode(self, language, task, kwargs, temperature, generation_config=None,
                 return_dict_in_generate=None) -> Union[torch.Tensor, MedusaGenerateOutput]:
@@ -594,6 +615,8 @@ class WhisperMedusaModel:
         output_scores = bool(kwargs.pop("output_scores", False))
         output_logits = bool(kwargs.pop("output_logits", False))
         as_dict = bool(return_dict_in_generate)
+        want_ns = as_dict and bool(kwargs.pop("output_no_speech_prob", False))
+        kwargs.pop("output_no_speech_prob", None)
         # engine option "scores" for this call: bit 0 = per-token log-probabilities (every dict result), bit 1 = the
         # scores rows.  0 without return_dict_in_generate: the loop then launches nothing extra.
         score_bits = (1 | (2 if output_scores or output_logits else 0)) if as_dict else 0
@@ -625,6 +648,10 @@ class WhisperMedusaModel:
         gp.tree_attention = 1 if kwargs.pop("tree_attention", False) else 0
         lib = _lib.load()
         _check(lib, self._handle, lib.wm_set_option(self._handle, b"scores", score_bits), "wm_set_option(scores)")
+        # engine option "no_speech_row" for this call (set on every call, like "scores": a host-side store, and a new
+        # engine after to() / close() starts with it off)
+        ns_row = self._no_speech_row(prompt, g) if want_ns else -1
+        _check(lib, self._handle, lib.wm_set_option(self._handle, b"no_speech_row", ns_row), "wm_set_option(no_speech_row)")
         tr = self._run_loop(prompt, gp)
         self.last_trace = tr
         self._last_medusa_temperature = float(gp.temperature)
@@ -632,7 +659,28 @@ class WhisperMedusaModel:
         sequences = torch.tensor([out], dtype=torch.long, device=self._device)
         if not as_dict:
             return sequences
-        return self._generate_output(sequences, tr, output_scores, output_logits)
+        out = self._generate_output(sequences, tr, output_scores, output_logits)
+        if want_ns:
+            prob = C.c_float(0.0)
+            token = int(g.no_timestamps_token_id) - 1      # HF's choice (generation_whisper.py _setup_no_speech_detection)
+            _check(lib, self._handle, lib.wm_last_no_speech(self._handle, token, C.byref(prob), None), "wm_last_no_speech")
+            out.no_speech_prob = float(prob.value)
+        return out
+
+    def _no_speech_row(self, prompt: Sequence[int], g) -> int:
+        """Index in the prompt of the start-of-transcript token, whose raw base-head row gives the no-speech
+        probability.  It must be among the rows the first iteration computes: the last ((n - 1) % 16) + 1 rows of a
+        prompt of n tokens (the leading 16-token chunks of a longer prompt are cached by prefill launches)."""
+        sot = int(g.decoder_start_token_id)
+        if getattr(g, "no_timestamps_token_id", None) is None:
+            raise ValueError("output_no_speech_prob needs the generation config's no_timestamps_token_id")
+        if sot not in prompt:
+            raise ValueError(f"output_no_speech_prob: the prompt has no start-of-transcript token ({sot})")
+        row = list(prompt).index(sot)
+        if row < (len(prompt) - 1) // 16 * 16:
+            raise NotImplementedError("output_no_speech_prob: the start-of-transcript token of a prompt longer than 16 "
+                                      "tokens must be among its last ((len - 1) % 16) + 1 tokens")
+        return row
 
     def _generate_output(self, sequences: torch.Tensor, tr: GenerateTrace, output_scores: bool,
                          output_logits: bool) -> MedusaGenerateOutput:
@@ -724,6 +772,17 @@ class WhisperMedusaModel:
         _check(lib, self._handle, lib.wm_last_logits(self._handle, which, C.cast(out.data_ptr(), C.POINTER(C.c_float))),
                "wm_last_logits")
         return out
+
+    def last_no_speech(self, token: Optional[int] = None) -> Tuple[float, torch.Tensor]:
+        """What the last ``generate(..., output_no_speech_prob=True)`` computed: ``p[token]`` (default: HF's no-speech
+        token, ``no_timestamps_token_id - 1``) and the raw base-head logits ``FloatTensor[V]`` of the SOT row."""
+        lib = _lib.load()
+        token = int(self.generation_config.no_timestamps_token_id) - 1 if token is None else int(token)
+        row = torch.empty(self.config.vocab_size, dtype=torch.float32)
+        prob = C.c_float(0.0)
+        _check(lib, self._handle, lib.wm_last_no_speech(self._handle, token, C.byref(prob),
+                                                        C.cast(row.data_ptr(), C.POINTER(C.c_float))), "wm_last_no_speech")
+        return float(prob.value), row
 
     def last_accept(self) -> Dict[str, Optional[Union[torch.Tensor, int]]]:
         """What the accept step of the last ``generate`` iteration compared (``wm_last_accept``), one entry per verify row
