@@ -67,9 +67,14 @@ def test_decode_logits_vs_fp64_reference(case):
     """Pass-A / pass-B logits of two speculative iterations and forward() logits, in every decode mode the width
     supports, against the fp64 oracle decoding from the engine's own encoder states.  Prints the error of the ring
     kernel (folded LayerNorm) over that of the explicit-LayerNorm modes."""
-    model, cfg, sd, pcm = _model(case)
-    cid = _case_id(case)
-    modes = _modes(case[0])
+    _logits_vs_fp64(_model(case), case[0], _case_id(case))
+
+
+def _logits_vs_fp64(entry, d, cid, bar=None):
+    """Pass-A / pass-B logits of iterations 1 and 2 and forward() logits in every decode mode of width ``d``, within
+    ``bar`` (default DECODE_LOGIT_BAR)."""
+    model, cfg, sd, pcm = entry
+    modes = _modes(d)
     model.set_decode_mode(modes[0])
     model.generate_from_pcm(pcm, max_iters=1, **_KW)
     enc = model.encoder_output()
@@ -90,9 +95,9 @@ def test_decode_logits_vs_fp64_reference(case):
             for ab, which in (("A", 0), ("B", 1)):
                 r64 = getattr(ref64, f"pass{ab}_logits")[it - 1].numpy()
                 r32 = getattr(ref32, f"pass{ab}_logits")[it - 1].numpy()
-                errs.append(check_logits(model.last_logits(which).numpy(), r64, cid, f"{mode}/pass{ab}{it}", r32))
+                errs.append(check_logits(model.last_logits(which).numpy(), r64, cid, f"{mode}/pass{ab}{it}", r32, bar))
         out = model.forward(decoder_input_ids=torch.tensor([ids])).logits.cpu()[:, 0].numpy()
-        errs.append(check_logits(out, fwd64, cid, f"{mode}/forward", fwd32))
+        errs.append(check_logits(out, fwd64, cid, f"{mode}/forward", fwd32, bar))
         worst[mode] = max(errs)
     explicit = max(worst[m] for m in ("persistent_simple", "graph"))
     ratio = f"{worst['persistent'] / explicit:.2f}" if "persistent" in worst and explicit > 0 else "n/a"

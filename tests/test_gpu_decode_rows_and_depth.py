@@ -135,7 +135,11 @@ def test_forward_sweeps_of_every_row_count(d):
     """forward() with the first 1..16 of 16 ids: a pass-A sweep of every row count a stage tile holds, every head at
     every position, in each decode mode of the width (and the ring on 8 and 37 CTAs at d = 512 / 1280).  The decoder is
     causal, so the fp64 reference of the first n ids is the first n rows of the 16-id reference."""
-    model, cfg, sd, pcm = _model(d, 4)
+    _forward_sweeps(_model(d, 4), d, f"A/d{d}")
+
+
+def _forward_sweeps(entry, d, cid):
+    model, cfg, sd, pcm = entry
     kw = dict(language=None, max_length=MAX_LEN)
     model.set_decode_mode(_modes(d)[0])
     enc = _engine_enc(model, pcm, kw)
@@ -151,7 +155,7 @@ def test_forward_sweeps_of_every_row_count(d):
             for n in range(1, 17):
                 out = model.forward(decoder_input_ids=torch.tensor([_FWD_IDS[:n]])).logits.cpu()[:, 0].numpy()
                 assert out.shape == (cfg.medusa_num_heads + 1, n, cfg.vocab_size)
-                check_logits(out, fwd64[:, :n], f"A/d{d}", f"{tag}/forward{n}", fwd32[:, :n])
+                check_logits(out, fwd64[:, :n], cid, f"{tag}/forward{n}", fwd32[:, :n])
     model.set_decode_mode(_modes(d)[0])
 
 
@@ -165,9 +169,16 @@ def test_chain_verify_sweeps_of_2_8_16_rows(case):
     d = 512, the ring elsewhere); then a whole generate to max_length 448 gives the tokens and accept lengths of the
     fp32 engine-regime oracle."""
     d, k, htype = case
-    model, cfg, sd, pcm = _model(d, k, heads_type=htype)
-    kw = dict(language=None, max_length=MAX_LEN)
     cid = f"B/d{d}-k{k}" + ("-block" if htype == "medusa_block" else "")
+    tr = _chain_verify_and_generate(_model(d, k, heads_type=htype), d, cid)
+    if k == 15 and htype == "base_head":
+        assert max(tr.accept_lengths) == 15, cid          # a 16-row verify sweep accepted whole
+
+
+def _chain_verify_and_generate(entry, d, cid):
+    """Two iterations against fp64, then a whole generate against the fp32 oracle; returns the generate's trace."""
+    model, cfg, sd, pcm = entry
+    kw = dict(language=None, max_length=MAX_LEN)
     runs = [(m, None) for m in (ALL_MODES if d == 512 else ("persistent",))]
     enc = _check_two_iterations(model, cfg, sd, pcm, kw, cid, runs)
     out = model.generate_from_pcm(pcm, **kw)[0].tolist()
@@ -178,8 +189,7 @@ def test_chain_verify_sweeps_of_2_8_16_rows(case):
     assert tr.sequences == ref.sequences, cid
     assert tr.accept_lengths == ref.accept_lengths, cid
     assert out == M.strip_output(ref.sequences, len(prompt), gp)
-    if k == 15 and htype == "base_head":
-        assert max(tr.accept_lengths) == 15, cid          # a 16-row verify sweep accepted whole
+    return tr
 
 
 # ---------------------------------------------------------------------------------------------------------------- C
@@ -213,7 +223,11 @@ def test_prefilled_prompts_to_full_depth(case):
     tokens against the fp64 oracle from the same prompt.  The ring at every width; every mode at 512 and 1280, and the
     ring on 8 and 37 CTAs at 1280."""
     d, k = case
-    model, cfg, sd, pcm = _model(d, k)
+    _prefilled_prompts(_model(d, k), d, k, f"D/d{d}-k{k}")
+
+
+def _prefilled_prompts(entry, d, k, cid):
+    model, cfg, sd, pcm = entry
     deepest = MAX_LEN - k - 2
     assert deepest + k == MAX_LEN - 2          # the last verify position is 446
     runs = [(m, None) for m in (ALL_MODES if d in (512, 1280) else ("persistent",))]
@@ -234,7 +248,7 @@ def test_prefilled_prompts_to_full_depth(case):
                 model.generate_from_pcm(pcm, max_iters=1, decoder_input_ids=torch.tensor([prompt]), **kw)
             tr = model.last_trace
             assert tr.iterations == 1 and tr.sequences == ref64.sequences, (n, tag)
-            _check_pass_logits(model, cfg, ref64, ref32, 1, f"D/d{d}-k{k}", f"{tag}/prompt{n}")
+            _check_pass_logits(model, cfg, ref64, ref32, 1, cid, f"{tag}/prompt{n}")
     model.set_decode_mode("persistent")
 
 
@@ -257,8 +271,11 @@ def test_logits_deep_in_the_real_loop(case):
     fp64 oracle started from the engine's own history, with the original prompt's begin-suppress index and
     length-penalty origin."""
     d, k, choices, ta, temp = case
-    model, cfg, sd, pcm = _model(d, k, choices)
-    cid = "E/" + _e_id(case)
+    _deep_in_the_loop(_model(d, k, choices), ta, temp, "E/" + _e_id(case))
+
+
+def _deep_in_the_loop(entry, ta, temp, cid):
+    model, cfg, sd, pcm = entry
     kw = dict(language=None, max_length=MAX_LEN, medusa_temperature=temp)
     model.set_decode_mode("persistent")
     model.generate_from_pcm(pcm, tree_attention=ta, **kw)

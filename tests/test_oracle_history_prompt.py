@@ -6,7 +6,11 @@ order.  One iteration of the fp64 oracle started from the loop's own history (pr
 iteration n), with the begin-suppress index and the length-penalty origin of the ORIGINAL prompt, recomputes that cache
 from the ids alone.  For chains and for ``tree_attention=True`` (every kept row was computed behind exactly its
 ancestors) it gives the same logits, to fp64 rounding, and the same tokens.  These runs go to a length of 400 and more,
-so the self-attention of the checked iterations spans hundreds of keys."""
+so the self-attention of the checked iterations spans hundreds of keys.
+
+The identity holds for Medusa-Block heads too: the block's K/V row at position p depends only on the decoder's
+final-LayerNorm state at p (the block's attention output is never cached), so recomputing it from the ids gives what the
+loop appended sweep by sweep."""
 import pytest
 import torch
 
@@ -17,13 +21,17 @@ from whisper_medusa_b200.synthetic import synthetic_audio, synthetic_state_dict,
 
 MAX_LEN = 448
 
-# (d_model, K, medusa_choices or None for the top-1 chain, tree_attention)
-CASES = [(128, 4, None, False), (128, 2, [1, 3, 4], True), (512, 15, None, False), (128, 3, [1, 3, 2, 1], True)]
+# (d_model, K, medusa_choices or None for the top-1 chain, tree_attention, heads type)
+CASES = [(128, 4, None, False, "base_head"), (128, 2, [1, 3, 4], True, "base_head"),
+         (512, 15, None, False, "base_head"), (128, 3, [1, 3, 2, 1], True, "base_head"),
+         (128, 4, None, False, "medusa_block"), (512, 15, None, False, "medusa_block"),
+         (128, 2, [1, 3, 4], True, "medusa_block"), (128, 3, [1, 3, 2, 1], True, "medusa_block")]
 
 
 def _case_id(case):
-    d, k, ch, ta = case
-    return f"d{d}-k{k}" + (f"-tree{''.join(map(str, ch))}" if ch else "") + ("-tree_attn" if ta else "")
+    d, k, ch, ta, ht = case
+    return f"d{d}-k{k}" + (f"-tree{''.join(map(str, ch))}" if ch else "") + ("-tree_attn" if ta else "") + \
+        ("-block" if ht == "medusa_block" else "")
 
 
 def _iter_lengths(prompt_len, accepts):
@@ -40,8 +48,8 @@ def _rel(a, b):
 
 @pytest.mark.parametrize("case", CASES, ids=_case_id)
 def test_one_iteration_from_the_history_equals_the_accumulated_run(case):
-    d, k, choices, tree_attn = case
-    cfg = width_config(d, heads=k)
+    d, k, choices, tree_attn, heads_type = case
+    cfg = width_config(d, heads=k, heads_type=heads_type)
     if choices:
         cfg.medusa_choices = list(choices)
     sd = synthetic_state_dict(cfg, seed=3)
