@@ -208,13 +208,21 @@ int wm_set_option(wm_handle* h, const char* key, int32_t value);
  * with on a GPU of n_sm SMs (0: 132) -- the shape with the fewest operand bytes on the busiest SM (DESIGN.md section 4).
  * fp16_out: the bias / bias+GELU epilogues; 0: the fp32 residual-stream epilogues (128 x 128 tiles only). */
 int wm_enc_gemm_tile(int32_t M, int32_t N, int32_t K, int32_t fp16_out, int32_t n_sm, int32_t* out3);
+/* Host logic, no GPU needed: replays the persistent decode kernel's weight ring for a decoder of width d_model (a
+ * multiple of 64), n_layers layers (+ the Medusa block if medusa_block), K heads and n_tree verify rows on n_cta CTAs,
+ * at every loop state a launch can start from (DESIGN.md section 3): the chunks the producer warp copies against the
+ * slots the compute warps take, CTA by CTA.  *n_bad = the number of (launch, CTA) pairs that differ, first4 = {kv_len,
+ * L, need_a, cta} of the first of them. */
+int wm_ring_schedule_check(int32_t d_model, int32_t n_layers, int32_t medusa_block, int32_t K, int32_t n_tree,
+                           int32_t n_cta, int32_t* n_bad, int32_t* first4);
 /* Debug: per-stage timeline of the last persistent iteration (after wm_set_option(h, "profile", 1)).
  * Rows of 24 int64: stage id, mode, layer; body ns and barrier-wait ns seen by the last CTA; then the
  * 16 raw probes of CTA 0 -- ns offsets from stage begin ([1] end of body, [2] end of barrier, [7] record
  * read, [8] activations landed, [9] LayerNorm statistics, [10] split done, [3] staged, [13] before the
  * weight wait, [4] weights present, [5] MMAs done, [6] epilogue done, [14] unit loop left, [15] stage
- * function left) and two flags ([11], [12]: weights already present at stage begin / before the wait);
- * 3 spare. */
+ * function left) and two flags ([11], [12]: weights already present at stage begin / before the wait;
+ * self-attention stages: its K prefix / its first V prefix block already in the ring at stage begin, also set when
+ * there is no prefix); 3 spare. */
 int wm_get_stage_profile(wm_handle* h, int64_t* out, int32_t cap_rows, int32_t* n_rows);
 
 #ifdef __cplusplus

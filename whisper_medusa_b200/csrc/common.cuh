@@ -33,12 +33,15 @@ struct DecTree {
 // one ring chunk: `nrows` (<= 16) rows of `copy_bytes` each, row r read at src + r * row_bytes and written at
 // slot + r * (slot row stride).  Weight chunks: rows of W (copy_bytes = d fp16); cross-attention chunks:
 // nrows = 1, one contiguous block of K or V rows.
+// nrows = 0: a self-attention prefix block whose size is known only at launch (sa_prefix_chunk): src = the layer's
+// self_k or self_v cache, block sa_block of the keys of the CTA's sa_item-th item in a pass of mode sa_mode.
 struct ChunkDesc {
   const void* src;
   uint32_t row_bytes;
   uint32_t nrows;
   uint32_t copy_bytes;
-  uint32_t pad_;
+  uint16_t sa_item;
+  uint8_t sa_mode, sa_block;
 };
 
 // One stage of the persistent ring kernel, fully resolved for one CTA by the host (built once per
@@ -172,6 +175,15 @@ __device__ __forceinline__ uint32_t pack_half2(float lo, float hi) {
   return *reinterpret_cast<uint32_t*>(&h);
 }
 
+// Self-attention K/V cache of a decoder layer: [H][WM_MAX_POS][72] fp16, head-major like the cross-attention K/V.  The
+// keys [0, n) of one head are one contiguous byte range (one bulk copy into a ring slot), and rows 144 B apart keep
+// the 16-byte shared-memory reads of the attention's per-thread dot products free of bank conflicts.
+#define WM_KV_ROW 72
+// element (position p, channel c = head * 64 + dim) of a self-K/V cache
+__host__ __device__ __forceinline__ size_t self_kv_index(int p, int c) {
+  return ((size_t)(c >> 6) * WM_MAX_POS + p) * WM_KV_ROW + (c & 63);
+}
+
 // ---------------------------------------------------------------------------------------
 // decode-side model description (lives in device memory; kernels take a pointer to it)
 // ---------------------------------------------------------------------------------------
@@ -191,8 +203,8 @@ struct DecLayer {
   const float* fc1_b;
   const __half* fc2_w;  // [d, ffn]
   const float* fc2_b;
-  __half* self_k;        // [WM_MAX_POS, d]
-  __half* self_v;        // [WM_MAX_POS, d]
+  __half* self_k;        // [H][WM_MAX_POS][72]: head-major, 64 dims + 8 halfs of padding per row (self_kv_index)
+  __half* self_v;        // [H][WM_MAX_POS][72]
   const __half* cross_k;   // [H][S_pad][72]: 64 dims + 8 halfs of padding (the shared-memory row of the attention kernels)
   const __half* cross_v;   // [H][S_pad][72]
 };

@@ -129,9 +129,9 @@ __device__ __forceinline__ void gemm_epilogue(const GemmDesc& g, int token, int 
       if (row < d) {
         g.out[(size_t)token * g.ldo + row] = v;
       } else if (row < 2 * d) {
-        g.kc[(size_t)(g.base + token) * d + (row - d)] = __float2half_rn(v);
+        g.kc[self_kv_index(g.base + token, row - d)] = __float2half_rn(v);
       } else {
-        g.vc[(size_t)(g.base + token) * d + (row - 2 * d)] = __float2half_rn(v);
+        g.vc[self_kv_index(g.base + token, row - 2 * d)] = __float2half_rn(v);
       }
       break;
     }
@@ -338,7 +338,8 @@ __device__ __noinline__ void stage_gemm(const GemmDesc& g, int cta, int ncta, un
 // -----------------------------------------------------------------------------------------
 // stage: causal self-attention over the fp16 cache (HF modeling_whisper.py:284-357, T_q <= 16)
 // item = (head, group of R query rows); R = ceil(H*T / n_cta) so that all items run in ONE wave.
-// Row t sees keys 0 .. base + t.  K/V rows come straight from L2 (the cache is small and hot).
+// Row t sees keys 0 .. base + t.  Stage kernels read the K/V rows straight from L2; the ring kernel takes the cached
+// prefix from ring slots (stage_self_attn_ring).
 // -----------------------------------------------------------------------------------------
 #define WM_SA_MAXR 4
 #ifndef WM_SA_PV_UNROLL
@@ -365,95 +366,148 @@ __device__ __forceinline__ float dot64_h(const float* q, const uint4* kp) {
   }
   return s;
 }
-template <bool SPLIT_OUT = false>
-__device__ __forceinline__ void stage_self_attn(const DecModel* m, int mode, int layer, int cta, int ncta, unsigned char* smem_raw, const PassGeom* gopt,
-                                                unsigned long long* pr = nullptr) {
-  const PassGeom g = gopt ? *gopt : pass_geom(m, mode);
-  const int d = m->d, H = m->H, T = g.T;
-  const DecLayer& L = m->layers[layer];
-  float* s_q = reinterpret_cast<float*>(smem_raw);                 // [R][64]
+// Items of the stage: item = (head, group of R query rows), R = ceil(H * T / ncta) within [1, WM_SA_MAXR]; item i is
+// head i / groups, rows from (i % groups) * R.
+struct SelfAttnSplit { int R, groups; };
+__host__ __device__ __forceinline__ SelfAttnSplit self_attn_split(int H, int T, int ncta) {
+  SelfAttnSplit s;
+  s.R = (H * T + ncta - 1) / ncta;
+  if (s.R > WM_SA_MAXR) s.R = WM_SA_MAXR;
+  if (s.R < 1) s.R = 1;
+  s.groups = (T + s.R - 1) / s.R;
+  return s;
+}
+
+// Ring kernel: the cached keys of a self-attention item that every row of the pass sees and that were written before
+// the launch, [0, min(base, kv0)), stream through the weight ring as blocks of up to WM_SA_BLOCK keys, a K and a V
+// chunk per block (at most WM_SA_BLOCKS, since WM_MAX_POS = 512).  Block `b` of the `k`-th item of CTA `cta` in a pass
+// of `mode`: head h, keys [j0, j0 + nk); nk = 0 when the item or the block does not exist at this launch's (L0, kv0).
+// The producer warp (which chunks it copies) and the compute warps (which slots they take) both decide from here.
+#define WM_SA_BLOCK 256
+#define WM_SA_BLOCKS (WM_MAX_POS / WM_SA_BLOCK)
+static_assert(WM_SA_BLOCK <= WM_CH_MAX_KEYS, "a self-attention prefix block must fit one ring slot, as a cross-attention chunk does");
+struct SaChunk { int h, j0, nk; };
+__host__ __device__ __forceinline__ SaChunk sa_prefix_chunk(int H, int ncta, int cta, int mode, int L0, int kv0, int n_tree,
+                                                            int k, int b) {
+  const PassGeom g = pass_geom(mode, L0, kv0, n_tree);
+  const SelfAttnSplit s = self_attn_split(H, g.T, ncta);
+  const int item = cta + k * ncta;
+  SaChunk c;
+  c.h = item / s.groups;
+  c.j0 = b * WM_SA_BLOCK;
+  const int n = min(g.base, kv0) - c.j0;
+  c.nk = (item < H * s.groups && n > 0) ? min(n, WM_SA_BLOCK) : 0;
+  return c;
+}
+
+// One (head, row group) item once its query rows are in s_q (and visible to the CTA).  Key j's row of K is loaded by
+// kload(j, a) into a[0..7] (its 64 dims), dims 8 dg .. 8 dg + 7 of V's row j by vload(j, dg).  after_qk runs once no
+// thread reads K any more, before_pv before the first read of V, after_pv once no thread reads V any more.
+template <bool SPLIT_OUT, class KLoad, class VLoad, class AfterQK, class BeforePV, class AfterPV>
+__device__ __forceinline__ void self_attn_item(const DecModel* m, const PassGeom& g, bool tree_mask, int h, int t0, int rg,
+                                               float* s_q, KLoad kload, VLoad vload, AfterQK after_qk, BeforePV before_pv,
+                                               AfterPV after_pv, unsigned long long* pr) {
+  const int d = m->d;
   float* s_p = s_q + WM_SA_MAXR * 64;                              // [R][WM_MAX_POS]
   float* s_st = s_p + WM_SA_MAXR * WM_MAX_POS;                     // [R] sum
   float* s_acc = s_st + 2 * WM_SA_MAXR;                            // [WM_DEC_THREADS / 8 groups][64]
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int nk_max = g.base + t0 + rg;           // keys of the last row of the group
+  // scores (scaled by head_dim^-0.5; HF scales q, a power of two, so this is identical)
+  const int npairs = rg * nk_max;
+  for (int i0 = tid; i0 < npairs; i0 += WM_DEC_THREADS) {
+    const int r0 = i0 / nk_max, j0 = i0 - r0 * nk_max;
+    uint4 a[8];
+    kload(j0, a);
+    bool ok0 = j0 <= g.base + t0 + r0;           // causal (over cache order: what the reference does for trees too)
+    if (tree_mask && j0 >= g.base) ok0 = ok0 && ((m->tree->anc[t0 + r0] >> (j0 - g.base)) & 1u);   // ancestors only
+    s_p[r0 * WM_MAX_POS + j0] = ok0 ? dot64_h(s_q + r0 * 64, a) * 0.125f : -INFINITY;
+  }
+  cta_sync();
+  after_qk();
+  if (pr) pr[4] = wm_timer_ns();
+  // softmax statistics: one warp per row
+  for (int r = warp; r < rg; r += (WM_DEC_THREADS >> 5)) {
+    const int nk = g.base + t0 + r + 1;
+    float* p = s_p + r * WM_MAX_POS;
+    float mx = -INFINITY;
+    for (int jj = lane; jj < nk; jj += 32) mx = fmaxf(mx, p[jj]);
+    mx = warp_max(mx);
+    float sum = 0.f;
+    for (int jj = lane; jj < nk; jj += 32) { const float e = expf(p[jj] - mx); p[jj] = e; sum += e; }
+    sum = warp_sum(sum);
+    if (lane == 0) s_st[r] = sum;
+  }
+  cta_sync();
+  if (pr) pr[5] = wm_timer_ns();
+  before_pv();
+  // P * V : thread = (row r, key group kg, dim group dg of 8 dims)
+  {
+    const int KG = (WM_DEC_THREADS / 8) / rg;
+    const int dg = tid & 7, gI = tid >> 3;       // groups of 8 threads
+    const int r = gI / KG, kg = gI - r * KG;
+    float a[8];
+#pragma unroll
+    for (int e = 0; e < 8; ++e) a[e] = 0.f;
+    if (r < rg) {
+      const int nk = g.base + t0 + r + 1;
+      const float* p = s_p + r * WM_MAX_POS;
+      WM_UNROLL(WM_SA_PV_UNROLL)
+      for (int jj = kg; jj < nk; jj += KG) {
+        const uint4 vv = vload(jj, dg);
+        const __half2* v2 = reinterpret_cast<const __half2*>(&vv);
+        const float pj = p[jj];
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          const float2 f = __half22float2(v2[e]);
+          a[2 * e] = fmaf(pj, f.x, a[2 * e]);
+          a[2 * e + 1] = fmaf(pj, f.y, a[2 * e + 1]);
+        }
+      }
+    }
+#pragma unroll
+    for (int e = 0; e < 8; ++e) s_acc[gI * 64 + dg * 8 + e] = a[e];
+    cta_sync();
+    after_pv();
+    if (pr) pr[6] = wm_timer_ns();
+    if (tid < rg * 64) {
+      const int rr = tid >> 6, c = tid & 63;
+      float o = 0.f;
+      for (int k2 = 0; k2 < KG; ++k2) o += s_acc[(rr * KG + k2) * 64 + c];
+      if (SPLIT_OUT) store_split(m->attn + (size_t)(t0 + rr) * d, h * 64 + c, o / s_st[rr]);   // (ring kernel: operand format of the O-projection)
+      else m->attn[(size_t)(t0 + rr) * d + h * 64 + c] = o / s_st[rr];
+    }
+  }
+}
+
+__device__ __forceinline__ void stage_self_attn(const DecModel* m, int mode, int layer, int cta, int ncta, unsigned char* smem_raw,
+                                                const PassGeom* gopt, unsigned long long* pr = nullptr) {
+  const PassGeom g = gopt ? *gopt : pass_geom(m, mode);
+  const int d = m->d, H = m->H;
+  const DecLayer& L = m->layers[layer];
+  float* s_q = reinterpret_cast<float*>(smem_raw);                 // [R][64], then the rest of self_attn_smem_bytes()
+  const int tid = threadIdx.x;
   const bool tree_mask = (mode == MODE_B) && m->has_tree && m->st->tree_attn;   // (tree_attn is constant during a generate call)
-  int R = (H * T + ncta - 1) / ncta;
-  if (R > WM_SA_MAXR) R = WM_SA_MAXR;
-  if (R < 1) R = 1;
-  const int groups = (T + R - 1) / R;
+  const SelfAttnSplit sp = self_attn_split(H, g.T, ncta);
+  const int R = sp.R, groups = sp.groups;
   for (int item = cta; item < H * groups; item += ncta) {
     const int h = item / groups, t0 = (item - h * groups) * R;
-    const int rg = min(R, T - t0);                 // rows in this group
-    const int nk_max = g.base + t0 + rg;           // keys of the last row of the group
+    const int rg = min(R, g.T - t0);               // rows in this group
     cta_sync();
     for (int idx = tid; idx < rg * 64; idx += WM_DEC_THREADS)
       s_q[idx] = ldcg_f(&m->q[(size_t)(t0 + (idx >> 6)) * d + h * 64 + (idx & 63)]);
     cta_sync();
     if (pr) pr[3] = wm_timer_ns();
-    // scores (scaled by head_dim^-0.5; HF scales q, a power of two, so this is identical)
-    const int npairs = rg * nk_max;
-    for (int i0 = tid; i0 < npairs; i0 += WM_DEC_THREADS) {
-      const int r0 = i0 / nk_max, j0 = i0 - r0 * nk_max;
-      const uint4* k0 = reinterpret_cast<const uint4*>(L.self_k + (size_t)j0 * d + h * 64);
-      uint4 a[8];
+    // K / V rows straight from L2
+    self_attn_item<false>(
+        m, g, tree_mask, h, t0, rg, s_q,
+        [&](int j, uint4* a) {
+          const uint4* k0 = reinterpret_cast<const uint4*>(L.self_k + self_kv_index(j, h * 64));
 #pragma unroll
-      for (int c = 0; c < 8; ++c) a[c] = ldcg_u4(k0 + c);
-      bool ok0 = j0 <= g.base + t0 + r0;           // causal (over cache order: what the reference does for trees too)
-      if (tree_mask && j0 >= g.base) ok0 = ok0 && ((m->tree->anc[t0 + r0] >> (j0 - g.base)) & 1u);   // ancestors only
-      s_p[r0 * WM_MAX_POS + j0] = ok0 ? dot64_h(s_q + r0 * 64, a) * 0.125f : -INFINITY;
-    }
-    cta_sync();
-    if (pr) pr[4] = wm_timer_ns();
-    // softmax statistics: one warp per row
-    for (int r = warp; r < rg; r += (WM_DEC_THREADS >> 5)) {
-      const int nk = g.base + t0 + r + 1;
-      float* p = s_p + r * WM_MAX_POS;
-      float mx = -INFINITY;
-      for (int jj = lane; jj < nk; jj += 32) mx = fmaxf(mx, p[jj]);
-      mx = warp_max(mx);
-      float sum = 0.f;
-      for (int jj = lane; jj < nk; jj += 32) { const float e = expf(p[jj] - mx); p[jj] = e; sum += e; }
-      sum = warp_sum(sum);
-      if (lane == 0) s_st[r] = sum;
-    }
-    cta_sync();
-    if (pr) pr[5] = wm_timer_ns();
-    // P * V : thread = (row r, key group kg, dim group dg of 8 dims)
-    {
-      const int KG = (WM_DEC_THREADS / 8) / rg;
-      const int dg = tid & 7, gI = tid >> 3;       // groups of 8 threads
-      const int r = gI / KG, kg = gI - r * KG;
-      float a[8];
-#pragma unroll
-      for (int e = 0; e < 8; ++e) a[e] = 0.f;
-      if (r < rg) {
-        const int nk = g.base + t0 + r + 1;
-        const float* p = s_p + r * WM_MAX_POS;
-        WM_UNROLL(WM_SA_PV_UNROLL)
-        for (int jj = kg; jj < nk; jj += KG) {
-          const uint4 vv = ldcg_u4(L.self_v + (size_t)jj * d + h * 64 + dg * 8);
-          const __half2* v2 = reinterpret_cast<const __half2*>(&vv);
-          const float pj = p[jj];
-#pragma unroll
-          for (int e = 0; e < 4; ++e) {
-            const float2 f = __half22float2(v2[e]);
-            a[2 * e] = fmaf(pj, f.x, a[2 * e]);
-            a[2 * e + 1] = fmaf(pj, f.y, a[2 * e + 1]);
-          }
-        }
-      }
-#pragma unroll
-      for (int e = 0; e < 8; ++e) s_acc[gI * 64 + dg * 8 + e] = a[e];
-      cta_sync();
-      if (pr) pr[6] = wm_timer_ns();
-      if (tid < rg * 64) {
-        const int rr = tid >> 6, c = tid & 63;
-        float o = 0.f;
-        for (int k2 = 0; k2 < KG; ++k2) o += s_acc[(rr * KG + k2) * 64 + c];
-        if (SPLIT_OUT) store_split(m->attn + (size_t)(t0 + rr) * d, h * 64 + c, o / s_st[rr]);   // (ring kernel: operand format of the O-projection)
-        else m->attn[(size_t)(t0 + rr) * d + h * 64 + c] = o / s_st[rr];
-      }
-    }
+          for (int c = 0; c < 8; ++c) a[c] = ldcg_u4(k0 + c);
+        },
+        [&](int j, int dg) { return ldcg_u4(L.self_v + self_kv_index(j, h * 64 + dg * 8)); },
+        [] {}, [] {}, [] {}, pr);
   }
 }
 
@@ -1223,7 +1277,8 @@ __device__ __noinline__ void stage_accept_tree(const DecModel* m, int ncta) {
 
 // stage: gather the surviving K/V rows of a tree verify pass to rows L .. L+keep-1 of every layer's cache (reference
 // model.py:383-401: tree_past[:, :, select_indices][..., :accept]).  One (layer, K|V) item per CTA turn; rows move in
-// path order (keep_src[j] >= L + j, so a row is always read before a later move can overwrite it).  No-op for chains.
+// path order (keep_src[j] >= L + j, so a row is always read before a later move can overwrite it), each as the 64
+// dims of every head (thread = head, 8 dims).  No-op for chains.
 __device__ __noinline__ void stage_kv_compact(const DecModel* m, int cta, int ncta) {
   const DecState* st = m->st;
   const int keep = ldcg_i(&st->keep_n);   // (written by CTA 0 in the previous stage: L2-coherent reads; uniform across the grid)
@@ -1231,18 +1286,17 @@ __device__ __noinline__ void stage_kv_compact(const DecModel* m, int cta, int nc
   const int d = m->d;
   const int n_l = m->n_layers + (m->has_block ? 1 : 0);
   const int L0 = ldcg_i(&st->keep_src[0]);   // = old L (node 0 is the root)
+  const bool on = threadIdx.x < d / 8;
+  const int c = 8 * threadIdx.x;   // channel of this thread's 8 dims
   for (int item = cta; item < 2 * n_l; item += ncta) {
     __half* base = (item & 1) ? m->layers[item >> 1].self_v : m->layers[item >> 1].self_k;
     for (int j = 1; j < keep; ++j) {
       const int src = ldcg_i(&st->keep_src[j]), dst = L0 + j;
       if (src != dst) {
-        const uint4* s4 = reinterpret_cast<const uint4*>(base + (size_t)src * d);
-        uint4* d4 = reinterpret_cast<uint4*>(base + (size_t)dst * d);
         uint4 v = make_uint4(0, 0, 0, 0);
-        const bool on = threadIdx.x < d / 8;
-        if (on) v = ldcg_u4(s4 + threadIdx.x);
+        if (on) v = ldcg_u4(base + self_kv_index(src, c));
         cta_sync();
-        if (on) d4[threadIdx.x] = v;
+        if (on) *reinterpret_cast<uint4*>(base + self_kv_index(dst, c)) = v;
       }
       cta_sync();
     }
@@ -1565,7 +1619,7 @@ void dec_build_ring_tables(const DecModel& hm, const float2* ln_fold, int ncta, 
     return g.bias;
   };
   auto push_chunk = [&](const void* src, size_t row_bytes, int nrows, size_t copy_bytes) {
-    ctab.push_back(ChunkDesc{src, (uint32_t)row_bytes, (uint32_t)nrows, (uint32_t)copy_bytes, 0u});
+    ctab.push_back(ChunkDesc{src, (uint32_t)row_bytes, (uint32_t)nrows, (uint32_t)copy_bytes, 0, 0, 0});
   };
   // LayerNorm gamma of the next instruction (bulk-copied into shared memory while this one runs)
   std::vector<const float*> nx_g(n, nullptr);
@@ -1610,6 +1664,21 @@ void dec_build_ring_tables(const DecModel& hm, const float2* ln_fold, int ncta, 
             push_chunk(L.cross_k + row0, 0, 1, it.nk * 72 * sizeof(__half));
             push_chunk(L.cross_v + row0, 0, 1, it.nk * 72 * sizeof(__half));
           }
+          continue;
+        }
+        if (stage == ST_SELF_ATTN) {
+          // per item of this CTA: its prefix blocks' K rows, then their V rows, sized at launch (sa_prefix_chunk).  A
+          // sweep-A pass has a row count known only at launch, so every item the CTA can get at some row count is listed.
+          const DecLayer& L = hm.layers[layer];
+          int items = 0;
+          for (int T = 1; T <= WM_MAX_T; ++T) {
+            const SelfAttnSplit sp = self_attn_split(hm.H, T, ncta);
+            items = std::max(items, (hm.H * sp.groups - cta + ncta - 1) / ncta);
+          }
+          for (int k = 0; k < items; ++k)
+            for (const __half* cache : {L.self_k, L.self_v})
+              for (int b = 0; b < WM_SA_BLOCKS; ++b)
+                ctab.push_back(ChunkDesc{cache, 0u, 0u, 0u, (uint16_t)k, (uint8_t)c.mode, (uint8_t)b});
           continue;
         }
         if (!is_gemm_stage(stage)) continue;
@@ -1660,6 +1729,102 @@ void dec_build_ring_tables(const DecModel& hm, const float2* ln_fold, int ncta, 
         }
       }
     }
+}
+
+// Host replay of the ring protocol (no GPU): for each CTA and each launch state, the chunks the producer warp copies
+// (ring_producer) against what the compute warps expect in the slots they take (stage_gemm_ring, stage_cross_attn_ring,
+// stage_self_attn_ring), compared as (source, rows, bytes).  Launch states: every kv0 in [0, WM_MAX_POS - 16] with sweep A
+// skipped (L0 = kv0), with sweep A over t_a = 1 ... 16 rows (L0 = kv0 + t_a), and prefill chunks of 16 rows; those whose
+// verify rows would pass WM_MAX_POS are left out.  Returns the number of (launch, CTA) pairs whose sequences differ;
+// `first` receives {kv0, L0, need_a, cta} of the first of them.
+int dec_check_ring_schedule(const DecModel& hm, int ncta, int first[4]) {
+  std::vector<CtaStage> stab;
+  std::vector<ChunkDesc> ctab;
+  std::vector<int> off;
+  const float2* fold = reinterpret_cast<const float2*>(uintptr_t(1) << 40);   // (never dereferenced)
+  dec_build_ring_tables(hm, fold, ncta, 1, stab, ctab, off);
+  std::vector<int> flat;
+  int poff[4];
+  dec_build_program(hm.n_layers, hm.has_block, flat, poff);
+  struct Copy {
+    const void* src; uint32_t nrows, bytes;
+    bool operator==(const Copy& o) const { return src == o.src && nrows == o.nrows && bytes == o.bytes; }
+  };
+  const uint32_t kv_bytes = WM_KV_ROW * sizeof(__half);
+  // what the GEMM and cross-attention stages of instruction ip take from the ring at CTA cta: fixed for every launch
+  std::vector<std::vector<Copy>> fixed((size_t)poff[3] * ncta);
+  for (int ip = 0; ip < poff[3]; ++ip) {
+    const int stage = flat[ip * 3], mode = flat[ip * 3 + 1], layer = flat[ip * 3 + 2];
+    const DecLayer& L = hm.layers[layer];
+    const PassGeom dyn{-1, 0};
+    if (stage == ST_CROSS_ATTN) {
+      for (int item = 0; item < hm.H * hm.cross_chunks; ++item) {
+        const CrossItem it = cross_item(item, hm.S, hm.cross_chunks);
+        if (it.nk == 0) continue;
+        const size_t row0 = ((size_t)it.h * hm.S_pad + it.j0) * 72;
+        std::vector<Copy>& f = fixed[(size_t)ip * ncta + item % ncta];
+        f.push_back(Copy{L.cross_k + row0, 1u, it.nk * kv_bytes});
+        f.push_back(Copy{L.cross_v + row0, 1u, it.nk * kv_bytes});
+      }
+    }
+    if (!is_gemm_stage(stage)) continue;
+    const GemmDesc g = make_gemm_desc(&hm, stage, mode, layer, &dyn);
+    for (int cta = 0; cta < ncta; ++cta) {
+      std::vector<Copy>& f = fixed[(size_t)ip * ncta + cta];
+      const CtaStage& sd = stab[(size_t)ip * ncta + cta];
+      for (int u = 0; u * 16 < sd.n_rows; ++u)
+        f.push_back(Copy{g.W + (size_t)(sd.n_begin + 16 * u) * g.K + (size_t)sd.seg * hm.d,
+                         (uint32_t)std::min(16, sd.n_rows - 16 * u), (uint32_t)(hm.d * sizeof(__half))});
+    }
+  }
+  std::vector<Copy> prod, cons;
+  int bad = 0;
+  auto run = [&](int L0, int kv0, int need_a, int prefill) {
+    for (int cta = 0; cta < ncta; ++cta) {
+      prod.clear();
+      cons.clear();
+      const int* o = &off[(size_t)cta * 4];
+      for (int c = need_a ? o[0] : o[1]; c < (prefill ? o[1] : o[3]); ++c) {
+        const ChunkDesc& dsc = ctab[c];
+        if (dsc.nrows != 0) { prod.push_back(Copy{dsc.src, dsc.nrows, dsc.copy_bytes}); continue; }
+        const SaChunk s = sa_prefix_chunk(hm.H, ncta, cta, dsc.sa_mode, L0, kv0, hm.n_tree, dsc.sa_item, dsc.sa_block);
+        if (s.nk == 0) continue;
+        prod.push_back(Copy{reinterpret_cast<const __half*>(dsc.src) + self_kv_index(s.j0, s.h * 64), 1u, s.nk * kv_bytes});
+      }
+      for (int ip = need_a ? poff[0] : poff[1]; ip < (prefill ? poff[1] : poff[3]); ++ip) {
+        const int stage = flat[ip * 3], mode = flat[ip * 3 + 1], layer = flat[ip * 3 + 2];
+        if (stage != ST_SELF_ATTN) {
+          const std::vector<Copy>& f = fixed[(size_t)ip * ncta + cta];
+          cons.insert(cons.end(), f.begin(), f.end());
+          continue;
+        }
+        const DecLayer& L = hm.layers[layer];
+        const PassGeom g = pass_geom(mode, L0, kv0, hm.n_tree);
+        const SelfAttnSplit sp = self_attn_split(hm.H, g.T, ncta);
+        int k = 0;
+        for (int item = cta; item < hm.H * sp.groups; item += ncta, ++k) {
+          const int h = item / sp.groups, P = std::min(g.base, kv0);
+          for (const __half* cache : {L.self_k, L.self_v})
+            for (int b = 0; b < WM_SA_BLOCKS; ++b) {
+              const SaChunk s = sa_prefix_chunk(hm.H, ncta, cta, mode, L0, kv0, hm.n_tree, k, b);
+              if (s.nk == 0) continue;
+              const int nk = std::min(WM_SA_BLOCK, P - b * WM_SA_BLOCK);   // the keys the stage reads from this slot
+              cons.push_back(Copy{cache + self_kv_index(b * WM_SA_BLOCK, h * 64), 1u, (uint32_t)nk * kv_bytes});
+            }
+        }
+      }
+      if (!(prod == cons)) {
+        if (bad++ == 0) { first[0] = kv0; first[1] = L0; first[2] = need_a; first[3] = cta; }
+      }
+    }
+  };
+  for (int kv0 = 0; kv0 <= WM_MAX_POS - 16; ++kv0) {
+    if (kv0 >= 1 && kv0 + hm.n_tree <= WM_MAX_POS) run(kv0, kv0, 0, 0);
+    for (int t_a = 1; t_a <= WM_MAX_T; ++t_a)
+      if (kv0 + t_a + hm.n_tree <= WM_MAX_POS) run(kv0 + t_a, kv0, 1, 0);
+    run(kv0 + 16, kv0, 1, 1);
+  }
+  return bad;
 }
 
 cudaError_t dec_relayout_cross_kv(const __half* kv, __half* ck, __half* cv, int S, int S_pad, int d, int H, cudaStream_t s,

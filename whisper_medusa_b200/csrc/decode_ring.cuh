@@ -38,8 +38,8 @@
 // rows.
 //
 // Ring geometry: a "chunk" = up to 16 weight rows x d columns (fp16), row stride d*2 + 64 B
-// (bank-conflict-free LDS.128 of the B fragments); WM_RING_G chunks are resident; chunks are
-// consumed in program order.
+// (bank-conflict-free LDS.128 of the B fragments), or the K or V rows of a cross-attention key chunk or of a
+// self-attention prefix block; WM_RING_G chunks are resident; chunks are consumed in program order.
 #pragma once
 
 #define WM_RING_G 3
@@ -148,6 +148,11 @@ __host__ __device__ constexpr int ring_nks(int d) {
 
 #define WM_XS_PADB 16   // bytes of X-row padding: stride = 16 (mod 128) => conflict-free LDS.128 / STS.128
 
+// Keys of a self-attention item that the ring does not bring (sa_prefix_chunk): the pass's own rows and those sweep A
+// wrote earlier in the launch, at most WM_MAX_T each.  Their K and V rows are staged behind the stage's scratch.
+#define WM_SA_NEW (2 * WM_MAX_T)
+__host__ __device__ constexpr size_t self_attn_new_rows_bytes() { return (size_t)2 * WM_SA_NEW * WM_KV_ROW * sizeof(__half); }
+
 template <int D>
 struct RingGeom {
   static_assert(D % 32 == 0 && D <= 1280, "decoder width must be a multiple of 32, at most 1280");
@@ -162,7 +167,8 @@ struct RingGeom {
   static constexpr int NV = (D + 127) / 128;          // float4 per lane of a row-per-warp pass
   // shared-memory map
   static constexpr size_t SCRATCH_OFF = (size_t)WM_RING_G * SLOT_BYTES;
-  static constexpr size_t SCRATCH = round128(cmax(cmax((size_t)16 * XS, cross_scratch_bytes()), self_attn_smem_bytes()));
+  static constexpr size_t SCRATCH =
+      round128(cmax(cmax((size_t)16 * XS, cross_scratch_bytes()), self_attn_smem_bytes() + self_attn_new_rows_bytes()));
   static constexpr size_t PARTIAL_OFF = SCRATCH_OFF + SCRATCH;
   static constexpr size_t PARTIAL = round128((size_t)NKS * 256 * sizeof(float));   // k-slice partials of one unit
   static constexpr size_t GAMMA_OFF = PARTIAL_OFF + PARTIAL;
@@ -176,9 +182,11 @@ struct RingGeom {
 // ---------------------------------------------------------------------------------------------
 // producer warp: stream the chunk table through the ring
 // ---------------------------------------------------------------------------------------------
+// (L0, kv0: the loop state at launch, which sizes the self-attention prefix chunks)
 template <int D>
 __device__ __noinline__ void ring_producer(unsigned char* ring, uint64_t* full, uint64_t* empty,
-                                           const ChunkDesc* __restrict__ tab, int first, int last) {
+                                           const ChunkDesc* __restrict__ tab, int first, int last, const DecModel* m,
+                                           int cta, int ncta, int L0, int kv0) {
   using G = RingGeom<D>;
   const int lane = threadIdx.x & 31;
   if (first >= last) return;
@@ -188,15 +196,25 @@ __device__ __noinline__ void ring_producer(unsigned char* ring, uint64_t* full, 
   for (int c = first; c < last; ++c) {
     const ChunkDesc dsc = nxt;
     if (c + 1 < last) nxt = tab[c + 1];                 // next descriptor is in flight while we wait
+    const unsigned char* src = reinterpret_cast<const unsigned char*>(dsc.src);
+    uint32_t nrows = dsc.nrows, copy_bytes = dsc.copy_bytes;
+    if (nrows == 0) {
+      // a self-attention prefix block: one contiguous copy of its K or V rows, or nothing (the consumer skips it too)
+      const SaChunk s = sa_prefix_chunk(m->H, ncta, cta, dsc.sa_mode, L0, kv0, m->n_tree, dsc.sa_item, dsc.sa_block);
+      if (s.nk == 0) continue;
+      src += self_kv_index(s.j0, s.h * 64) * sizeof(__half);
+      nrows = 1;
+      copy_bytes = (uint32_t)s.nk * WM_KV_ROW * sizeof(__half);
+    }
     if (lane == 0) {
       while (!mbar_try_wait(empty + slot, par)) { }
       asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic reads of the slot vs async writes
-      mbar_expect_tx(full + slot, dsc.nrows * dsc.copy_bytes);
+      mbar_expect_tx(full + slot, nrows * copy_bytes);
     }
     __syncwarp();
-    if (lane < dsc.nrows) {
-      bulk_g2s(ring + (size_t)slot * G::SLOT_BYTES + (size_t)lane * G::ROW_STRIDE,
-               reinterpret_cast<const unsigned char*>(dsc.src) + (size_t)lane * dsc.row_bytes, dsc.copy_bytes, full + slot);
+    if (lane < nrows) {
+      bulk_g2s(ring + (size_t)slot * G::SLOT_BYTES + (size_t)lane * G::ROW_STRIDE, src + (size_t)lane * dsc.row_bytes,
+               copy_bytes, full + slot);
     }
     __syncwarp();
     if (++slot == WM_RING_G) { slot = 0; par ^= 1u; }
@@ -508,8 +526,8 @@ __device__ __forceinline__ void stage_gemm_ring(RingState& rs, unsigned char* sm
           const float v = y;
           const DecLayer& L = m->layers[sd->layer];
           if (row < D) out[(size_t)token * ldo + row] = v;
-          else if (row < 2 * D) L.self_k[(size_t)(base + token) * D + (row - D)] = __float2half_rn(v);
-          else L.self_v[(size_t)(base + token) * D + (row - 2 * D)] = __float2half_rn(v);
+          else if (row < 2 * D) L.self_k[self_kv_index(base + token, row - D)] = __float2half_rn(v);
+          else L.self_v[self_kv_index(base + token, row - 2 * D)] = __float2half_rn(v);
         } else if (epi == EPI_HEADS_A) {
           // head `row / d` on the newest token's hidden state: x + SiLU(W x + b)  (medusa ResBlock)
           const int head = row / D, n = row - head * D;
@@ -608,6 +626,101 @@ __device__ __forceinline__ void stage_cross_attn_ring(RingState& rs, unsigned ch
   }
 }
 
+// ---------------------------------------------------------------------------------------------
+// self-attention fed from the ring: the keys [0, P) of each item, P = min(base, kv0), arrive as K chunks and then V
+// chunks of up to WM_SA_BLOCK keys (sa_prefix_chunk), streamed while QKV and its barrier run.  Only the query rows and
+// the keys [P, nk_max) (the pass's own rows, and those sweep A wrote in this launch) come from L2, in one round, into
+// the staging rows behind the scratch.  Items, the thread of each (row, key) pair and every sum are those of
+// stage_self_attn, so the results are the same bits.
+// ---------------------------------------------------------------------------------------------
+template <int D>
+__device__ __forceinline__ void stage_self_attn_ring(RingState& rs, unsigned char* smem, const DecModel* m, int mode, int layer,
+                                                     int cta, int ncta, const PassGeom& g, int L0, int kv0,
+                                                     unsigned long long* pr) {
+  using G = RingGeom<D>;
+  uint64_t* const full = reinterpret_cast<uint64_t*>(smem + G::BAR_OFF);
+  uint64_t* const empty = full + WM_RING_G;
+  float* const s_q = reinterpret_cast<float*>(smem + G::SCRATCH_OFF);
+  __half* const sKn = reinterpret_cast<__half*>(smem + G::SCRATCH_OFF + self_attn_smem_bytes());   // [WM_SA_NEW][72]
+  __half* const sVn = sKn + WM_SA_NEW * WM_KV_ROW;
+  const int H = m->H;
+  const DecLayer& L = m->layers[layer];
+  const int tid = threadIdx.x;
+  const bool tree_mask = (mode == MODE_B) && m->has_tree && m->st->tree_attn;
+  const SelfAttnSplit sp = self_attn_split(H, g.T, ncta);
+  const int P = min(g.base, kv0);
+  int k = 0;
+  for (int item = cta; item < H * sp.groups; item += ncta, ++k) {
+    const int h = item / sp.groups, t0 = (item - h * sp.groups) * sp.R;
+    const int rg = min(sp.R, g.T - t0);
+    const int nnew = g.base + t0 + rg - P;
+    // ring chunks of the item: nb K blocks, then nb V blocks, in consecutive slots
+    int nb = 0;
+    for (int b = 0; b < WM_SA_BLOCKS; ++b)
+      if (sa_prefix_chunk(H, ncta, cta, mode, L0, kv0, m->n_tree, k, b).nk > 0) nb = b + 1;
+    auto slot_of = [&](int i, unsigned int& par) {
+      const int s = rs.slot + i;
+      par = rs.par ^ (s >= WM_RING_G ? 1u : 0u);
+      return s >= WM_RING_G ? s - WM_RING_G : s;
+    };
+    unsigned int pk0, pk1;
+    const __half* const sK0 = reinterpret_cast<const __half*>(smem + (size_t)slot_of(0, pk0) * G::SLOT_BYTES);
+    const __half* const sK1 = reinterpret_cast<const __half*>(smem + (size_t)slot_of(1, pk1) * G::SLOT_BYTES);
+    unsigned int pv0, pv1;
+    const __half* const sV0 = reinterpret_cast<const __half*>(smem + (size_t)slot_of(nb, pv0) * G::SLOT_BYTES);
+    const __half* const sV1 = reinterpret_cast<const __half*>(smem + (size_t)slot_of(nb + 1, pv1) * G::SLOT_BYTES);
+    if (pr && k == 0) {
+      pr[11] = (nb == 0 || mbar_try_wait(full + slot_of(nb - 1, pk1), pk1)) ? 1000ull : 0ull;   // K prefix here at begin?
+      pr[12] = (nb == 0 || mbar_try_wait(full + slot_of(nb, pv0), pv0)) ? 1000ull : 0ull;       // first V block?
+    }
+    cta_sync();   // (the previous item's readers of the scratch are done)
+    for (int idx = tid; idx < rg * 64; idx += WM_DEC_THREADS)
+      s_q[idx] = ldcg_f(&m->q[(size_t)(t0 + (idx >> 6)) * D + h * 64 + (idx & 63)]);
+    // 16 bytes per thread: (row, K | V, 8 dims)
+    for (int idx = tid; idx < nnew * 16; idx += WM_DEC_THREADS) {
+      const int r = idx >> 4, v = (idx >> 3) & 1, c = (idx & 7) * 8;
+      const __half* src = (v ? L.self_v : L.self_k) + self_kv_index(P + r, h * 64 + c);
+      *reinterpret_cast<uint4*>((v ? sVn : sKn) + r * WM_KV_ROW + c) = ldcg_u4(src);
+    }
+    cta_sync();
+    if (pr) pr[3] = global_timer_ns();
+    for (int i = 0; i < nb; ++i) {
+      unsigned int p;
+      const int s = slot_of(i, p);
+      while (!mbar_try_wait(full + s, p)) { }
+    }
+    auto row = [&](const __half* s0, const __half* s1, const __half* sn, int j) {
+      return j < P ? (j < WM_SA_BLOCK ? s0 + j * WM_KV_ROW : s1 + (j - WM_SA_BLOCK) * WM_KV_ROW) : sn + (j - P) * WM_KV_ROW;
+    };
+    self_attn_item<true>(
+        m, g, tree_mask, h, t0, rg, s_q,
+        [&](int j, uint4* a) {
+          const uint4* k0 = reinterpret_cast<const uint4*>(row(sK0, sK1, sKn, j));
+#pragma unroll
+          for (int c = 0; c < 8; ++c) a[c] = k0[c];
+        },
+        [&](int j, int dg) { return *reinterpret_cast<const uint4*>(row(sV0, sV1, sVn, j) + dg * 8); },
+        [&] {
+          if (tid == 0)
+            for (int i = 0; i < nb; ++i) { unsigned int p; mbar_arrive_n(empty + slot_of(i, p), G::NKS); }
+        },
+        [&] {
+          for (int i = nb; i < 2 * nb; ++i) {
+            unsigned int p;
+            const int s = slot_of(i, p);
+            while (!mbar_try_wait(full + s, p)) { }
+          }
+        },
+        [&] {
+          if (tid == 0)
+            for (int i = nb; i < 2 * nb; ++i) { unsigned int p; mbar_arrive_n(empty + slot_of(i, p), G::NKS); }
+        },
+        pr);
+    for (int i = 0; i < 2 * nb; ++i)
+      if (++rs.slot == WM_RING_G) { rs.slot = 0; rs.par ^= 1u; }
+  }
+}
+
 template <int D, bool PROF>
 __global__ void __launch_bounds__(WM_RING_THREADS, 1)
 dec_iteration_ring_kernel(const DecModel* __restrict__ gm) {
@@ -646,7 +759,8 @@ dec_iteration_ring_kernel(const DecModel* __restrict__ gm) {
   if (warp == WM_DEC_THREADS / 32) {
     // ===== producer warp =====
     const int* off = m->chunk_off + cta * 4;
-    ring_producer<D>(smem, full, empty, m->chunk_tab, need_a ? off[0] : off[1], st->prefill ? off[1] : off[3]);
+    ring_producer<D>(smem, full, empty, m->chunk_tab, need_a ? off[0] : off[1], st->prefill ? off[1] : off[3], m, cta, ncta,
+                     L0, kv0);
     return;
   }
 
@@ -690,7 +804,7 @@ dec_iteration_ring_kernel(const DecModel* __restrict__ gm) {
     } else if (stage == ST_CROSS_ATTN) {
       stage_cross_attn_ring<D>(rs, smem, m, pgv.T, cta, ncta, pr);
     } else if (stage == ST_SELF_ATTN) {
-      stage_self_attn<true>(m, mode, sd->layer, cta, ncta, smem + G::SCRATCH_OFF, &pgv, pr);
+      stage_self_attn_ring<D>(rs, smem, m, mode, sd->layer, cta, ncta, pgv, L0, kv0, pr);
     } else {
       run_stage<false>(m, stage, mode, sd->layer, cta, ncta, smem + G::SCRATCH_OFF, &pgv, pr);
     }

@@ -307,8 +307,8 @@ extern "C" int wm_create(const wm_config* cfg, int device, wm_handle** out) {
   for (int i = 0; i < h->n_dec; ++i) {
     CK(dalloc(&h->cross_k[i], (size_t)c.n_heads * SP * 72));
     CK(dalloc(&h->cross_v[i], (size_t)c.n_heads * SP * 72));
-    CK(dalloc(&h->self_k[i], (size_t)WM_MAX_POS * d));
-    CK(dalloc(&h->self_v[i], (size_t)WM_MAX_POS * d));
+    CK(dalloc(&h->self_k[i], (size_t)c.n_heads * WM_MAX_POS * WM_KV_ROW));
+    CK(dalloc(&h->self_v[i], (size_t)c.n_heads * WM_MAX_POS * WM_KV_ROW));
   }
   {
     std::vector<float> fb = build_mel_filters(80);
@@ -1277,6 +1277,31 @@ extern "C" int wm_enc_gemm_tile(int32_t M, int32_t N, int32_t K, int32_t fp16_ou
   int t[3];
   enc_gemm_tc_tile(M, N, K, fp16_out != 0, n_sm, t);
   out3[0] = t[0]; out3[1] = t[1]; out3[2] = t[2];
+  return WM_OK;
+}
+extern "C" int wm_ring_schedule_check(int32_t d_model, int32_t n_layers, int32_t medusa_block, int32_t K, int32_t n_tree,
+                                      int32_t n_cta, int32_t* n_bad, int32_t* first4) {
+  if (!n_bad || !first4 || d_model < 64 || d_model % 64 != 0 || n_layers < 1 || n_layers + 1 > WM_MAX_DEC_LAYERS || K < 1 ||
+      n_tree < 1 || n_tree > WM_MAX_T || n_cta < 4 || n_cta > 1024)
+    return WM_ERR_INVALID;
+  // a model description whose buffers are distinct placeholder addresses (the replay compares addresses, never reads)
+  uintptr_t next = uintptr_t(1) << 44;
+  auto fake = [&next](auto& p) { p = reinterpret_cast<std::remove_reference_t<decltype(p)>>(next); next += uintptr_t(1) << 32; };
+  DecModel m;
+  memset(&m, 0, sizeof m);
+  m.d = d_model; m.H = d_model / 64; m.ffn = 4 * d_model; m.V = 51865; m.S = 1500; m.S_pad = 1536;
+  m.n_layers = n_layers; m.has_block = medusa_block ? 1 : 0; m.K = K; m.n_tree = n_tree; m.has_tree = n_tree != K + 1;
+  m.cross_chunks = std::min(WM_CROSS_CHUNKS, std::max((m.S + WM_CH_MAX_KEYS - 1) / WM_CH_MAX_KEYS, n_cta / m.H));
+  for (int i = 0; i < n_layers + m.has_block; ++i) {
+    DecLayer& L = m.layers[i];
+    fake(L.ln1_g); fake(L.ln1_b); fake(L.qkv_w); fake(L.qkv_b); fake(L.o_w); fake(L.o_b); fake(L.ln2_g); fake(L.ln2_b);
+    fake(L.cq_w); fake(L.cq_b); fake(L.co_w); fake(L.co_b); fake(L.ln3_g); fake(L.ln3_b); fake(L.fc1_w); fake(L.fc1_b);
+    fake(L.fc2_w); fake(L.fc2_b); fake(L.self_k); fake(L.self_v); fake(L.cross_k); fake(L.cross_v);
+  }
+  fake(m.embed); fake(m.pos); fake(m.lnf_g); fake(m.lnf_b); fake(m.heads_w); fake(m.heads_b);
+  fake(m.x); fake(m.xg); fake(m.q); fake(m.attn); fake(m.ffn_h); fake(m.hidden); fake(m.head_h); fake(m.carry);
+  for (int i = 0; i < 4; ++i) first4[i] = -1;
+  *n_bad = dec_check_ring_schedule(m, n_cta, first4);
   return WM_OK;
 }
 extern "C" void* wm_weights_device_ptr(wm_handle* h) { return (h && h->wready) ? (void*)h->wdev : nullptr; }
