@@ -155,6 +155,32 @@ int wm_last_scores(wm_handle* h, float* token_logprobs, int32_t cap, int32_t* n_
  * did not capture the SOT row (the capture buffer is set to NaN before every such loop).  wm_forward never captures. */
 int wm_last_no_speech(wm_handle* h, int32_t token, float* prob, float* row_logits);
 
+/* ---- token-level timestamps (HF generate(return_token_timestamps=True), _extract_token_timestamps) ---------- */
+/* Alignment heads: pairs[2 i] = decoder layer (< decoder_layers), pairs[2 i + 1] = head (< heads), n_pairs <= 64, in
+ * HF's order; a pair listed twice counts twice.  While n_pairs > 0, every wm_generate keeps the raw cross-attention
+ * scores of those heads at every position its passes compute (the last pass to compute a position wins: for a chain,
+ * the one that accepted its token).  The capture buffer is allocated on first use (n distinct pairs x 528 x S floats).
+ * n_pairs = 0: capture off (the default).  wm_forward never captures. */
+int wm_set_alignment_heads(wm_handle* h, const int32_t* pairs, int32_t n_pairs);
+/* Token timestamps of the last wm_generate's sequence, cut to its first n_total ids (prompt of n_prompt ids included):
+ * timestamps (n_total floats) = [0] * n_prompt, then the DTW time of rows n_prompt .. n_total - 2, then that last time
+ * again.  num_frames: the clip's feature frames (the columns are cropped to num_frames / 2), or -1 (all S);
+ * filter_width: the median filter (odd); time_precision: seconds per encoder frame.  matrix (N x F floats, N = n_total -
+ * 1 - n_prompt, F the cropped width) and jumps (N ints: the frame each row starts at) may be NULL.  WM_ERR_STATE if the
+ * last wm_generate captured nothing (or the pairs changed since); WM_ERR_UNSUPPORTED on a branching tree. */
+int wm_token_timestamps(wm_handle* h, int32_t n_prompt, int32_t n_total, int32_t num_frames, int32_t filter_width,
+                        double time_precision, float* timestamps, float* matrix, int32_t* jumps);
+/* The same extraction on caller-provided probability rows probs [n_heads][n_rows][width] (host): timestamps receives
+ * n_prompt + n_rows + 1 floats.  n_rows <= 448 and a cropped width <= 1500. */
+int wm_token_timestamps_from_probs(wm_handle* h, const float* probs, int32_t n_heads, int32_t n_rows, int32_t width,
+                                   int32_t n_prompt, int32_t num_frames, int32_t filter_width, double time_precision,
+                                   float* timestamps, float* matrix, int32_t* jumps);
+/* The captured rows row0 .. row0 + n_rows - 1 of the last wm_generate as cross-attention probabilities (softmax over
+ * all S frames): out [pairs][n_rows][S], cap = its capacity in floats (WM_ERR_INVALID when too small).  Rows must lie
+ * in [0, L - 1) of the last sequence (L = its length).  n_pairs (may be NULL) receives the number of pairs the last
+ * wm_generate captured; out = NULL only reports it. */
+int wm_last_alignment_probs(wm_handle* h, int32_t row0, int32_t n_rows, float* out, int64_t cap, int32_t* n_pairs);
+
 /* ---- teacher-forced forward (model.py:1223-1347 `forward(...).logits`, shape [K+1, 1, T, V]) -------------- */
 /* ids: 1..16 decoder_input_ids; out (host, capacity (K+1) * n_ids * vocab_size floats) receives the raw logits of
  * every head at every position, out[(k * n_ids + t) * V + v]; k = 0 is the base head.  Needs wm_encode_* first. */

@@ -171,6 +171,8 @@ class MedusaConfig:
         base.setdefault("max_target_positions", 448)
         base.setdefault("activation_function", "gelu")
         base.setdefault("scale_embedding", False)
+        # width of the median filter applied to the alignment heads' weights for token timestamps (HF WhisperConfig)
+        base.setdefault("median_filter_width", 7)
         for k, v in base.items():
             setattr(self, k, v)
         if self.medusa_heads_type not in ("base_head", "medusa_block"):
@@ -233,6 +235,9 @@ class MedusaGenerationConfig:
         self.temperature = kwargs.pop("temperature", 1.0)
         self.num_beams = kwargs.pop("num_beams", 1)
         self.do_sample = kwargs.pop("do_sample", False)
+        # [[layer, head], ...] cross-attention heads whose weights align tokens with audio frames (token timestamps); a
+        # checkpoint brings them in its generation_config.json.  None: not available (saved only when set).
+        self.alignment_heads = kwargs.pop("alignment_heads", None)
         self._extra = kwargs
 
     def update(self, **kwargs: Any) -> None:
@@ -242,6 +247,8 @@ class MedusaGenerationConfig:
 
     def to_dict(self) -> Dict[str, Any]:
         d = {k: copy.deepcopy(v) for k, v in self.__dict__.items() if not k.startswith("_")}
+        if d.get("alignment_heads") is None:
+            d.pop("alignment_heads", None)
         return d
 
     def save_pretrained(self, path: str) -> None:

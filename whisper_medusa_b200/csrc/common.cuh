@@ -297,6 +297,19 @@ struct alignas(16) DecModel {   // (copied to shared memory in 16-byte pieces by
   // sweep A (row index within that pass's tile, prefill chunks excluded) into ns_hidden [d]; -1 = off
   float* ns_hidden;
   int ns_row;
+  // token-timestamp capture (wm_set_alignment_heads): null = off (it then costs one predicate per cross-attention item)
+  const struct TsCapture* ts;
+};
+
+// Token-timestamp capture.  The cross-attention stages of the base decoder layers store, for every alignment head, the
+// raw scores (q . k / 8, fp32, before the softmax) of each row r < T of passes A and B at the row's position:
+// scores[slot][position][S].  A position is written again by every pass that recomputes it, so the last writer is the
+// pass that accepted its token (DESIGN.md section 7).
+#define WM_TS_ROWS (WM_MAX_POS + WM_MAX_T)
+#define WM_TS_MAX_HEADS 32
+struct TsCapture {
+  float* scores;                                  // [n_slots][WM_TS_ROWS][S]
+  int slot[WM_MAX_DEC_LAYERS * WM_TS_MAX_HEADS];  // [layer * H + head]: capture slot, -1 = not captured
 };
 
 }  // namespace wm

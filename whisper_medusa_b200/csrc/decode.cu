@@ -608,10 +608,35 @@ __device__ __forceinline__ void cross_attn_fold(const DecModel* m, int T, int h,
   }
 }
 
-template <bool SPLIT_OUT, class AfterQK, class AfterPV>
+// Token-timestamp capture of one (head, key chunk) item (out of line: the rare branch adds no registers to the stage):
+// when `layer` is a base decoder layer, the pass is A or B and head h is an alignment head, warp r copies the nk raw
+// scores of row r < T to the row's position (chain: base + r; tree: base + depth).  Ends in a CTA barrier, so the
+// softmax that follows may overwrite the scores in place.
+__device__ __noinline__ void ts_capture(const DecModel* m, int mode, int layer, int T, int h, int c, int nch, int nk,
+                                        const float* sS) {
+  if (mode == MODE_TAIL || layer >= m->n_layers) return;
+  const TsCapture* ts = m->ts;
+  const int slot = ts->slot[layer * m->H + h];
+  if (slot < 0) return;
+  const int base = (mode == MODE_A) ? ldcg_i(&m->st->kv_len) : ldcg_i(&m->st->L);
+  const int j0 = cross_item(h * nch + c, m->S, nch).j0;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  for (int r = warp; r < T; r += (WM_DEC_THREADS >> 5)) {
+    const int pos = base + ((mode == MODE_B && m->has_tree) ? m->tree->depth[r] : r);
+    if (pos >= WM_TS_ROWS) continue;
+    float* dst = ts->scores + ((size_t)slot * WM_TS_ROWS + pos) * m->S + j0;
+    for (int j = lane; j < nk; j += 32) dst[j] = sS[r * WM_SS_STRIDE + j];
+  }
+  cta_sync();
+}
+
+// `on_scores(sS)` runs when token-timestamp capture is on (m->ts), after S = Q K^T is complete and before the softmax
+// overwrites it: the caller binds the pass mode and layer (ts_capture).
+template <bool SPLIT_OUT, class AfterQK, class AfterPV, class OnScores>
 __device__ __forceinline__ void cross_attn_core(const DecModel* m, int T, int h, int c, int nch, int nk, int nk_pad,
                                                 const __half* sK, const __half* sV, const CrossScratch& cs,
-                                                AfterQK&& after_qk, AfterPV&& after_pv, unsigned long long* pr = nullptr) {
+                                                AfterQK&& after_qk, AfterPV&& after_pv, OnScores&& on_scores,
+                                                unsigned long long* pr = nullptr) {
   __shared__ int s_last;
   float* sS = cs.sS; __half* sQh = cs.sQh; __half* sQl = cs.sQl; float* sM = cs.sM;
   const int d = m->d;
@@ -658,6 +683,7 @@ __device__ __forceinline__ void cross_attn_core(const DecModel* m, int T, int h,
   cta_sync();
   if (pr) pr[5] = wm_timer_ns();
   after_qk();
+  if (m->ts != nullptr) on_scores(sS);
   // ---- per-row max / exp / sum : warp per row, two keys per lane; rows >= T and keys >= nk become zero
   // probability.  The probabilities replace the scores IN PLACE as the fp16 operand pairs of the P V MMAs:
   // floats (p[2j], p[2j+1]) -> { half2 hi, half2 lo }, so the 8 warps of the next phase do not each redo the split.
@@ -772,7 +798,8 @@ __device__ __forceinline__ void stage_cross_attn(const DecModel* m, int mode, in
       reinterpret_cast<uint4*>(sK)[nk * 9 + idx] = make_uint4(0, 0, 0, 0);
       reinterpret_cast<uint4*>(sV)[nk * 9 + idx] = make_uint4(0, 0, 0, 0);
     }
-    cross_attn_core<false>(m, g.T, h, c, nch, nk, nk_pad, sK, sV, cs, [] {}, [] {});
+    cross_attn_core<false>(m, g.T, h, c, nch, nk, nk_pad, sK, sV, cs, [] {}, [] {},
+                           [&](const float* s) { ts_capture(m, mode, layer, g.T, h, c, nch, nk, s); });
   }
 }
 

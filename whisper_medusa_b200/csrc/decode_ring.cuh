@@ -590,8 +590,8 @@ __device__ __forceinline__ void stage_gemm_ring(RingState& rs, unsigned char* sm
 // read them in place (the cache rows already have the 72-half shared-memory stride).
 // ---------------------------------------------------------------------------------------------
 template <int D>
-__device__ __forceinline__ void stage_cross_attn_ring(RingState& rs, unsigned char* smem, const DecModel* m, int T, int cta, int ncta,
-                                                      unsigned long long* pr) {
+__device__ __forceinline__ void stage_cross_attn_ring(RingState& rs, unsigned char* smem, const DecModel* m, const CtaStage* sd,
+                                                      int T, int cta, int ncta, unsigned long long* pr) {
   using G = RingGeom<D>;
   uint64_t* const full = reinterpret_cast<uint64_t*>(smem + G::BAR_OFF);
   uint64_t* const empty = full + WM_RING_G;
@@ -622,7 +622,8 @@ __device__ __forceinline__ void stage_cross_attn_ring(RingState& rs, unsigned ch
     cross_attn_core<true>(
         m, T, h, c, nch, nk, nk_pad, sK, sV, cs,
         [&] { if (tid == 0) mbar_arrive_n(empty + slot_k, G::NKS); },
-        [&] { if (tid == 0) mbar_arrive_n(empty + slot_v, G::NKS); }, pr);
+        [&] { if (tid == 0) mbar_arrive_n(empty + slot_v, G::NKS); },
+        [&](const float* s) { ts_capture(m, sd->mode, sd->layer, T, h, c, nch, nk, s); }, pr);
   }
 }
 
@@ -802,7 +803,7 @@ dec_iteration_ring_kernel(const DecModel* __restrict__ gm) {
     if (is_gemm_stage(stage)) {
       stage_gemm_ring<D>(rs, smem, m, sd, pgv.T, pgv.base, pr);
     } else if (stage == ST_CROSS_ATTN) {
-      stage_cross_attn_ring<D>(rs, smem, m, pgv.T, cta, ncta, pr);
+      stage_cross_attn_ring<D>(rs, smem, m, sd, pgv.T, cta, ncta, pr);
     } else if (stage == ST_SELF_ATTN) {
       stage_self_attn_ring<D>(rs, smem, m, mode, sd->layer, cta, ncta, pgv, L0, kv0, pr);
     } else {

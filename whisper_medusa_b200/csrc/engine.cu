@@ -115,7 +115,21 @@ struct wm_handle {
   float* ns_part = nullptr;     // [WM_NS_NSEG][2] segment partials, then [1] log-sum-exp
   unsigned int* ns_count = nullptr;
   int last_ns = 0;              // 1: the last wm_generate computed the row
+  // token timestamps (wm_set_alignment_heads); buffers allocated on first use, the capture grown with the pair count
+  std::vector<int> ts_list;     // listed pairs as layer * H + head, in order (duplicates kept)
+  int ts_slot_cap = 0;          // slots the capture buffer holds
+  TsCapture* ts_dev = nullptr;  // device capture description (DecModel::ts while capture is on)
+  float* ts_scores = nullptr;   // [ts_slot_cap][WM_TS_ROWS][S]
+  int* ts_head_slot = nullptr;  // [WM_TS_MAX_LIST] capture slot of each listed pair
+  float* ts_probs = nullptr;    // [listed pairs][N][width] row probabilities, normalised in place by the extraction
+  size_t ts_probs_cap = 0;
+  float* ts_matrix = nullptr;   // [WM_TS_MAX_N][WM_TS_MAX_F]
+  int* ts_jumps = nullptr;      // [WM_TS_MAX_N]
+  float* ts_times = nullptr;    // [WM_TS_MAX_N + 1]
+  int last_ts = 0, last_ts_tree = 0;   // 1: the last wm_generate captured the listed pairs (on a branching tree)
 };
+
+#define WM_TS_MAX_LIST 64   // alignment pairs per call (duplicates included)
 
 static_assert(offsetof(DecState, tree_attn) == 60, "the 16 header words of DecState (L .. tree_attn) are patched as one 64-byte copy");
 
@@ -398,6 +412,7 @@ extern "C" int wm_destroy(wm_handle* h) {
   F(h->hm.topk_part); F(h->tree); F(h->hm.logits_a); F(h->hm.logits_b); F(h->st); F(h->tok_mask); F(h->pen_tab); F(h->bar); F(h->prof); F(h->chunk_tab); F(h->chunk_off); F(h->stage_tab); F(h->ln_fold); F(h->dm);
   F(h->score_state); F(h->score_part); F(h->score_lp); F(h->score_rows);
   F(h->hm.ns_hidden); F(h->ns_head); F(h->ns_logits); F(h->ns_part); F(h->ns_count);
+  F(h->ts_dev); F(h->ts_scores); F(h->ts_head_slot); F(h->ts_probs); F(h->ts_matrix); F(h->ts_jumps); F(h->ts_times);
   if (h->wowned) F(h->wdev);
   for (auto& kv : h->resamplers) { F(kv.second.taps); F(kv.second.sup); }
   if (h->h_state) cudaFreeHost(h->h_state);
@@ -849,6 +864,16 @@ static int set_ns_row(wm_handle* h, int row) {
   return WM_OK;
 }
 
+// Token-timestamp capture on / off (DecModel::ts): changes the device copy in stream order when it differs.
+static int set_ts_capture(wm_handle* h, bool on) {
+  const TsCapture* want = on ? h->ts_dev : nullptr;
+  if (want == h->hm.ts) return WM_OK;
+  h->hm.ts = want;
+  CK(cudaMemcpyAsync(reinterpret_cast<char*>(h->dm) + offsetof(DecModel, ts), &h->hm.ts, sizeof(h->hm.ts),
+                     cudaMemcpyHostToDevice, h->stream));
+  return WM_OK;
+}
+
 extern "C" int wm_generate(wm_handle* h, const int32_t* prompt, int32_t n_prompt, const wm_gen_params* gp,
                            int32_t* out_ids, int32_t* n_out, int32_t* accept_lens, int32_t* n_iter) {
   if (!h || !prompt || !gp || !out_ids || !n_out) return WM_ERR_INVALID;
@@ -871,6 +896,11 @@ extern "C" int wm_generate(wm_handle* h, const int32_t* prompt, int32_t n_prompt
   h->last_score_bits = 0;
   h->st_from_generate = 0;
   h->last_ns = 0;
+  h->last_ts = 0;
+  {
+    const int r = set_ts_capture(h, !h->ts_list.empty());
+    if (r != WM_OK) return r;
+  }
   {
     const int r = set_ns_row(h, h->ns_prompt_row >= 0 ? h->ns_prompt_row - ns_tail0 : -1);
     if (r != WM_OK) return r;
@@ -1010,6 +1040,168 @@ extern "C" int wm_generate(wm_handle* h, const int32_t* prompt, int32_t n_prompt
   h->last_score_bits = score_bits; h->last_prompt = n_prompt; h->last_L = L; h->last_iters = iters;
   h->st_from_generate = 1;
   h->last_ns = h->hm.ns_row >= 0;
+  h->last_ts = h->hm.ts != nullptr;
+  h->last_ts_tree = h->hm.has_tree;
+  return WM_OK;
+}
+
+extern "C" int wm_set_alignment_heads(wm_handle* h, const int32_t* pairs, int32_t n_pairs) {
+  if (!h || n_pairs < 0 || (n_pairs > 0 && !pairs)) return WM_ERR_INVALID;
+  if (n_pairs > WM_TS_MAX_LIST) return fail(h, WM_ERR_INVALID, "at most 64 alignment pairs");
+  const int H = h->cfg.n_heads;
+  std::vector<int> list(n_pairs);
+  for (int i = 0; i < n_pairs; ++i) {
+    const int l = pairs[2 * i], hd = pairs[2 * i + 1];
+    if (l < 0 || l >= h->cfg.dec_layers) return fail(h, WM_ERR_INVALID, "alignment head layer out of range (0 <= layer < decoder_layers)");
+    if (hd < 0 || hd >= H) return fail(h, WM_ERR_INVALID, "alignment head out of range (0 <= head < decoder_attention_heads)");
+    list[i] = l * H + hd;
+  }
+  if (list == h->ts_list) return WM_OK;
+  if (h->device < 0) return fail(h, WM_ERR_STATE, "layout-only handle");
+  if (H > WM_TS_MAX_HEADS) return fail(h, WM_ERR_UNSUPPORTED, "more than 32 attention heads");
+  CK(cudaSetDevice(h->device));
+  CK(cudaStreamSynchronize(h->stream));   // (no loop may read the table while it is rewritten)
+  h->last_ts = 0;
+  h->ts_list = list;
+  if (n_pairs == 0) return WM_OK;   // wm_generate switches the capture off
+  // one capture slot per distinct pair, in order of first appearance
+  std::vector<int> slot_of(h->cfg.dec_layers * H, -1), list_slot(n_pairs);
+  int n_slots = 0;
+  for (int i = 0; i < n_pairs; ++i) {
+    if (slot_of[list[i]] < 0) slot_of[list[i]] = n_slots++;
+    list_slot[i] = slot_of[list[i]];
+  }
+  if (!h->ts_dev) {
+    CK(dalloc(&h->ts_dev, 1));
+    CK(dalloc(&h->ts_head_slot, WM_TS_MAX_LIST));
+    CK(dalloc(&h->ts_matrix, (size_t)WM_TS_MAX_N * WM_TS_MAX_F));
+    CK(dalloc(&h->ts_jumps, WM_TS_MAX_N));
+    CK(dalloc(&h->ts_times, WM_TS_MAX_N + 1));
+  }
+  if (n_slots > h->ts_slot_cap) {
+    if (h->ts_scores) CK(cudaFree(h->ts_scores));
+    h->ts_scores = nullptr;
+    h->ts_slot_cap = 0;
+    CK(dalloc(&h->ts_scores, (size_t)n_slots * WM_TS_ROWS * h->S));
+    h->ts_slot_cap = n_slots;
+  }
+  std::vector<TsCapture> tc(1);
+  tc[0].scores = h->ts_scores;
+  for (int i = 0; i < WM_MAX_DEC_LAYERS * WM_TS_MAX_HEADS; ++i) tc[0].slot[i] = -1;
+  for (int i = 0; i < h->cfg.dec_layers * H; ++i) tc[0].slot[i] = slot_of[i];
+  CK(cudaMemcpy(h->ts_dev, tc.data(), sizeof(TsCapture), cudaMemcpyHostToDevice));
+  CK(cudaMemcpy(h->ts_head_slot, list_slot.data(), (size_t)n_pairs * sizeof(int), cudaMemcpyHostToDevice));
+  return WM_OK;
+}
+
+static int ts_probs_reserve(wm_handle* h, size_t elems) {
+  if (elems <= h->ts_probs_cap) return WM_OK;
+  if (h->ts_probs) CK(cudaFree(h->ts_probs));
+  h->ts_probs = nullptr;
+  h->ts_probs_cap = 0;
+  CK(dalloc(&h->ts_probs, elems));
+  h->ts_probs_cap = elems;
+  return WM_OK;
+}
+
+// The extraction on ts_probs ([n_heads][N][ldp], already filled) -> out [n_prompt + N + 1], matrix [N][F], jumps [N]
+static int ts_extract(wm_handle* h, int n_heads, int N, int ldp, int F, int n_prompt, int filter, double time_precision,
+                      float* out, float* matrix, int32_t* jumps) {
+  for (int i = 0; i < n_prompt + N + 1; ++i) out[i] = 0.f;
+  if (N <= 0) return WM_OK;   // HF: no row after the prompt => all zeros
+  TsExtractArgs a;
+  a.probs = h->ts_probs; a.ldp = ldp; a.n_heads = n_heads; a.N = N; a.F = F; a.filter = filter;
+  a.time_precision = time_precision; a.matrix = h->ts_matrix; a.jumps = h->ts_jumps; a.times = h->ts_times;
+  CK(ts_launch_extract(a, h->stream, nullptr));
+  CK(cudaMemcpyAsync(out + n_prompt, h->ts_times, (size_t)(N + 1) * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
+  if (matrix && F > 0)
+    CK(cudaMemcpyAsync(matrix, h->ts_matrix, (size_t)N * F * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
+  if (jumps) CK(cudaMemcpyAsync(jumps, h->ts_jumps, (size_t)N * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+  CK(cudaStreamSynchronize(h->stream));
+  return WM_OK;
+}
+
+static int ts_check_filter(wm_handle* h, int filter) {
+  if (filter <= 0 || filter % 2 != 1) return fail(h, WM_ERR_INVALID, "`filter_width` should be an odd number");
+  if (filter > WM_TS_MAX_FILTER) return fail(h, WM_ERR_UNSUPPORTED, "filter_width above 31");
+  return WM_OK;
+}
+
+extern "C" int wm_token_timestamps(wm_handle* h, int32_t n_prompt, int32_t n_total, int32_t num_frames, int32_t filter_width,
+                                   double time_precision, float* timestamps, float* matrix, int32_t* jumps) {
+  if (!h || !timestamps) return WM_ERR_INVALID;
+  if (!h->last_ts) return fail(h, WM_ERR_STATE, "the last wm_generate captured no alignment heads (wm_set_alignment_heads)");
+  if (h->last_ts_tree) return fail(h, WM_ERR_UNSUPPORTED, "token timestamps need a chain (branching medusa_choices)");
+  if (n_prompt < 0 || n_total < n_prompt + 1 || n_total > h->last_L)
+    return fail(h, WM_ERR_INVALID, "need 0 <= n_prompt < n_total <= the last sequence's length");
+  {
+    const int r = ts_check_filter(h, filter_width);
+    if (r != WM_OK) return r;
+  }
+  const int N = n_total - 1 - n_prompt;
+  if (N > WM_TS_MAX_N) return fail(h, WM_ERR_UNSUPPORTED, "more than 448 rows");
+  const int F = num_frames < 0 ? h->S : std::min(h->S, num_frames / 2);
+  const int nh = (int)h->ts_list.size();
+  CK(cudaSetDevice(h->device));
+  if (N > 0) {
+    const int r = ts_probs_reserve(h, (size_t)nh * N * h->S);
+    if (r != WM_OK) return r;
+    TsSoftmaxArgs sa;
+    sa.scores = h->ts_scores; sa.head_slot = h->ts_head_slot; sa.n_heads = nh; sa.S = h->S; sa.row0 = n_prompt; sa.N = N;
+    sa.probs = h->ts_probs;
+    CK(ts_launch_softmax(sa, h->stream));
+  }
+  return ts_extract(h, nh, N, h->S, F, n_prompt, filter_width, time_precision, timestamps, matrix, jumps);
+}
+
+extern "C" int wm_token_timestamps_from_probs(wm_handle* h, const float* probs, int32_t n_heads, int32_t n_rows, int32_t width,
+                                              int32_t n_prompt, int32_t num_frames, int32_t filter_width, double time_precision,
+                                              float* timestamps, float* matrix, int32_t* jumps) {
+  if (!h || !timestamps || (n_heads * n_rows * width > 0 && !probs)) return WM_ERR_INVALID;
+  if (n_heads < 1 || n_rows < 0 || width < 0 || n_prompt < 0) return fail(h, WM_ERR_INVALID, "bad shape");
+  {
+    const int r = ts_check_filter(h, filter_width);
+    if (r != WM_OK) return r;
+  }
+  const int F = num_frames < 0 ? width : std::min(width, num_frames / 2);
+  if (n_rows > WM_TS_MAX_N || F > WM_TS_MAX_F) return fail(h, WM_ERR_UNSUPPORTED, "more than 448 rows or 1500 frames");
+  if (h->device < 0) return fail(h, WM_ERR_STATE, "layout-only handle");
+  CK(cudaSetDevice(h->device));
+  if (!h->ts_matrix) {
+    CK(dalloc(&h->ts_matrix, (size_t)WM_TS_MAX_N * WM_TS_MAX_F));
+    CK(dalloc(&h->ts_jumps, WM_TS_MAX_N));
+    CK(dalloc(&h->ts_times, WM_TS_MAX_N + 1));
+  }
+  const size_t n = (size_t)n_heads * n_rows * width;
+  if (n > 0) {
+    const int r = ts_probs_reserve(h, n);
+    if (r != WM_OK) return r;
+    CK(cudaMemcpyAsync(h->ts_probs, probs, n * sizeof(float), cudaMemcpyHostToDevice, h->stream));
+  }
+  return ts_extract(h, n_heads, n_rows, width, F, n_prompt, filter_width, time_precision, timestamps, matrix, jumps);
+}
+
+extern "C" int wm_last_alignment_probs(wm_handle* h, int32_t row0, int32_t n_rows, float* out, int64_t cap,
+                                       int32_t* n_pairs) {
+  if (!h) return WM_ERR_INVALID;
+  if (!h->last_ts) return fail(h, WM_ERR_STATE, "the last wm_generate captured no alignment heads (wm_set_alignment_heads)");
+  const int nh = (int)h->ts_list.size();
+  if (n_pairs) *n_pairs = nh;
+  if (!out) return WM_OK;
+  // positions 0 .. L-2 of the last sequence are rows of accepted tokens; L-1 (and beyond) may not have been computed
+  if (row0 < 0 || n_rows < 1 || row0 + n_rows > h->last_L - 1)
+    return fail(h, WM_ERR_INVALID, "rows must lie in [0, L - 1) of the last sequence");
+  const size_t need = (size_t)nh * n_rows * h->S;
+  if (cap < 0 || (size_t)cap < need) return fail(h, WM_ERR_INVALID, "out holds fewer than pairs x n_rows x S floats");
+  CK(cudaSetDevice(h->device));
+  const int r = ts_probs_reserve(h, need);
+  if (r != WM_OK) return r;
+  TsSoftmaxArgs sa;
+  sa.scores = h->ts_scores; sa.head_slot = h->ts_head_slot; sa.n_heads = nh; sa.S = h->S; sa.row0 = row0; sa.N = n_rows;
+  sa.probs = h->ts_probs;
+  CK(ts_launch_softmax(sa, h->stream));
+  CK(cudaMemcpyAsync(out, h->ts_probs, need * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
+  CK(cudaStreamSynchronize(h->stream));
   return WM_OK;
 }
 
@@ -1081,7 +1273,11 @@ extern "C" int wm_forward(wm_handle* h, const int32_t* ids, int32_t n_ids, float
   const size_t V = (size_t)h->cfg.vocab_size;
   h->st_from_generate = 0;   // the loop state is rewritten below
   {
-    const int r = set_ns_row(h, -1);   // (the passes below must not overwrite the last wm_generate's captured row)
+    const int r = set_ts_capture(h, false);   // (the passes below must not overwrite the last wm_generate's captured
+    if (r != WM_OK) return r;                  //  alignment rows, nor its no-speech row)
+  }
+  {
+    const int r = set_ns_row(h, -1);
     if (r != WM_OK) return r;
   }
   for (int t = 1; t <= n_ids; ++t) {

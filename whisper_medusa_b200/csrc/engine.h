@@ -91,6 +91,31 @@ struct NoSpeechArgs {
 // product), 1 for medusa_block, and adds them to *n_launch
 cudaError_t dec_launch_no_speech(const NoSpeechArgs& a, int grid, cudaStream_t s, int64_t* n_launch);
 
+// ---- timestamps.cu ----
+#define WM_TS_MAX_FILTER 31    // widest median filter
+#define WM_TS_MAX_N 448        // DTW rows (the trace of 448 x 1500 cells is 168 KB of shared memory)
+#define WM_TS_MAX_F 1500       // DTW columns
+// Row softmax of captured scores: probs[head][i][0..S) for rows row0 .. row0 + N - 1 of the slot of each listed head.
+struct TsSoftmaxArgs {
+  const float* scores;     // TsCapture::scores [slots][WM_TS_ROWS][S]
+  const int* head_slot;    // [n_heads] device: slot of each listed (layer, head) pair, duplicates allowed
+  int n_heads, S, row0, N;
+  float* probs;            // [n_heads][N][S]
+};
+cudaError_t ts_launch_softmax(const TsSoftmaxArgs& a, cudaStream_t s);
+// Normalise, median-filter, average over heads, DTW and backtrace (HF _extract_token_timestamps after the crop).
+struct TsExtractArgs {
+  float* probs;            // [n_heads][N][ldp]: row probabilities; columns < F are normalised in place
+  int ldp, n_heads, N, F, filter;
+  double time_precision;
+  float* matrix;           // [N][F]
+  int* jumps;              // [N]: frame of the first DTW cell of each row (-1 when the path enters the row at frame 0)
+  float* times;            // [N + 1]: f32(jump * time_precision), then the last one repeated
+};
+size_t ts_dtw_smem_bytes(int N, int F);
+// enqueues 3 kernels (1 when F = 0) and adds them to *n_launch (may be null)
+cudaError_t ts_launch_extract(const TsExtractArgs& a, cudaStream_t s, int64_t* n_launch);
+
 // ---- mel.cu ----
 // pcm: device f32 [480000] (already zero padded). Outputs: mel_f32 [80][3000], xT fp16 [rows>=3000+?][80]
 // time-major with one leading zero row (conv padding); gmax_bits: device scratch (1 int).

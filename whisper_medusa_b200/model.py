@@ -24,6 +24,7 @@ from __future__ import annotations
 
 import ctypes as C
 import os
+import warnings
 from typing import Dict, List, Optional, Sequence, Tuple, Union
 
 import numpy as np
@@ -119,14 +120,20 @@ class MedusaGenerateOutput:
     * ``accept_lengths``: the accept length of every iteration;
     * ``no_speech_prob`` (``output_no_speech_prob=True``, else ``None``): the probability of ``<|nospeech|>``
       (``no_timestamps_token_id - 1``) in the softmax of the raw base-head logits at the start-of-transcript position
-      (HF ``WhisperNoSpeechDetection``), computed on the GPU (``csrc/no_speech.cu``); a float.
+      (HF ``WhisperNoSpeechDetection``), computed on the GPU (``csrc/no_speech.cu``); a float;
+    * ``token_timestamps`` (``return_token_timestamps=True``, else ``None``): ``FloatTensor[1, n]``, the time in seconds
+      of every id of ``sequences[0]`` (HF ``_extract_token_timestamps``: DTW over the alignment heads' cross-attention),
+      computed on the GPU (``csrc/timestamps.cu``).  Without ``return_dict_in_generate`` it is the only field besides
+      ``sequences``.
 
     Fields are attributes and keys (``out.scores`` / ``out["scores"]``); an integer indexes the fields that are not
     ``None``, in the order above, as HF ``ModelOutput`` does."""
 
-    FIELDS = ("sequences", "scores", "logits", "token_logprobs", "avg_logprob", "accept_lengths", "no_speech_prob")
+    FIELDS = ("sequences", "scores", "logits", "token_logprobs", "avg_logprob", "accept_lengths", "no_speech_prob",
+              "token_timestamps")
 
-    def __init__(self, sequences, scores, logits, token_logprobs, avg_logprob, accept_lengths, no_speech_prob=None):
+    def __init__(self, sequences, scores, logits, token_logprobs, avg_logprob, accept_lengths, no_speech_prob=None,
+                 token_timestamps=None):
         self.sequences = sequences
         self.scores = scores
         self.logits = logits
@@ -134,6 +141,7 @@ class MedusaGenerateOutput:
         self.avg_logprob = avg_logprob
         self.accept_lengths = accept_lengths
         self.no_speech_prob = no_speech_prob
+        self.token_timestamps = token_timestamps
 
     def keys(self) -> List[str]:
         return [k for k in self.FIELDS if getattr(self, k) is not None]
@@ -444,7 +452,13 @@ class WhisperMedusaModel:
         (reference ``model.py:1419-1779``); returns ``LongTensor[1, n]``, or with ``return_dict_in_generate=True`` a
         ``MedusaGenerateOutput`` (``output_scores`` / ``output_logits`` / ``output_no_speech_prob`` select its
         ``scores`` / ``logits`` / ``no_speech_prob``; without ``return_dict_in_generate`` they have no effect, as in HF
-        and the reference).  ``no_speech_threshold`` raises as in the reference: the skip rule is ``transcribe``'s."""
+        and the reference).  ``no_speech_threshold`` raises as in the reference: the skip rule is ``transcribe``'s.
+
+        ``return_token_timestamps=True``: token-level timestamps as HF computes them (``_extract_token_timestamps`` with
+        the generation config's ``alignment_heads``, ``config.median_filter_width`` and ``time_precision``), in
+        ``token_timestamps`` of a ``MedusaGenerateOutput`` (the only other field is ``sequences`` unless
+        ``return_dict_in_generate``).  ``attention_mask`` (the feature extractor's, ``[1, 3000]``) crops the alignment to
+        the clip's frames.  Chains of ``medusa_choices`` only."""
         self._require_engine()
         if input_features is None:
             raise ValueError("input_features is required")
@@ -464,8 +478,55 @@ class WhisperMedusaModel:
         if input_features.shape[-1] != N_FRAMES or input_features.shape[-2] != self.config.num_mel_bins:
             raise ValueError(f"input_features must be [1, {self.config.num_mel_bins}, {N_FRAMES}] (WhisperProcessor output)")
         self._check_unsupported(temperature, attention_mask, kwargs)
+        num_frames = self._mask_frames(attention_mask) if attention_mask is not None else None
+        ts = self._timestamp_request(generation_config, task, num_frames, time_precision) if return_token_timestamps else None
         self._encode_features(input_features)
-        return self._decode(language, task, kwargs, temperature, generation_config, return_dict_in_generate)
+        return self._decode(language, task, kwargs, temperature, generation_config, return_dict_in_generate,
+                            **({"token_timestamps": ts} if ts else {}))
+
+    @staticmethod
+    def _mask_frames(attention_mask) -> int:
+        """Frame count of the clip (HF ``attention_mask.sum(-1)``) from a one-row feature-extractor mask, ``[1, 3000]``
+        or ``[3000]``.  A mask of several rows belongs to a batch: ``generate`` takes one clip, so it raises rather than
+        crop this clip by another row (``StreamGroup.generate`` hands each row its own mask)."""
+        mask = torch.as_tensor(attention_mask)
+        if mask.dim() == 2 and mask.shape[0] == 1:
+            mask = mask[0]
+        if mask.dim() != 1 or mask.shape[0] != N_FRAMES:
+            raise ValueError(f"attention_mask must be one clip's mask, [1, {N_FRAMES}] or [{N_FRAMES}], got shape "
+                             f"{tuple(torch.as_tensor(attention_mask).shape)} (for a batch, use StreamGroup.generate)")
+        return int(mask.sum())
+
+    @staticmethod
+    def pcm_num_frames(n_samples: int) -> int:
+        """Feature frames of a clip of ``n_samples`` 16 kHz samples: the ``attention_mask.sum(-1)`` of
+        ``WhisperFeatureExtractor(..., return_attention_mask=True)`` (one frame per started hop of 160 samples)."""
+        return min(N_FRAMES, (int(n_samples) + 159) // 160)
+
+    def _timestamp_request(self, generation_config, task, num_frames: Optional[int],
+                           time_precision: float) -> Tuple[Optional[int], float]:
+        """Checks of ``return_token_timestamps=True`` before any GPU work (HF ``_set_num_frames`` / ``_median_filter``);
+        returns ``(num_frames, time_precision)`` for ``_decode``."""
+        g = generation_config if generation_config is not None else self.generation_config
+        if (task or getattr(g, "task", None)) == "translate":
+            warnings.warn("Token-level timestamps may not be reliable for task 'translate'.")
+        heads = getattr(g, "alignment_heads", None)
+        if heads is None:
+            raise ValueError(
+                "Model generation config has no `alignment_heads`, token-level timestamps not available. "
+                "See https://gist.github.com/hollance/42e32852f24243b748ae6bc1f985b13a on how to add this property to the generation config.")
+        for pair in heads:
+            l, h = (int(v) for v in pair)
+            if not (0 <= l < self.config.decoder_layers and 0 <= h < self.config.decoder_attention_heads):
+                raise ValueError(f"alignment head {[l, h]} is out of range: {self.config.decoder_layers} decoder layers of "
+                                 f"{self.config.decoder_attention_heads} heads")
+        width = int(getattr(self.config, "median_filter_width", 7))
+        if width <= 0 or width % 2 != 1:
+            raise ValueError("`filter_width` should be an odd number")
+        if any(int(c) != 1 for c in self.config.medusa_choices):
+            raise NotImplementedError("return_token_timestamps needs a chain of medusa_choices (all 1): the verify rows of "
+                                      "a branching tree are not the rows of one decoded sequence")
+        return num_frames, float(time_precision)
 
     def _encode_features(self, input_features: torch.Tensor) -> None:
         lib = _lib.load()
@@ -500,12 +561,19 @@ class WhisperMedusaModel:
 
     def generate_from_pcm(self, pcm: Union[np.ndarray, torch.Tensor], language: Optional[str] = None,
                           task: Optional[str] = None, temperature=None, sampling_rate: int = SAMPLE_RATE,
-                          return_dict_in_generate=None, **kwargs) -> Union[torch.Tensor, MedusaGenerateOutput]:
+                          return_dict_in_generate=None, return_token_timestamps=None, time_precision: float = 0.02,
+                          **kwargs) -> Union[torch.Tensor, MedusaGenerateOutput]:
         """Same as ``generate`` but takes mono f32 PCM and runs the log-mel frontend on the GPU
         (what ``WhisperProcessor`` does on the CPU in the reference's caller, eval_whisper_medusa.py:46-51).
         ``sampling_rate`` other than 16000 (any positive integer rate): the clip is uploaded and resampled to 16 kHz on
-        the GPU first (``torchaudio.functional.resample`` with its defaults); the 30 s limit applies after resampling."""
+        the GPU first (``torchaudio.functional.resample`` with its defaults); the 30 s limit applies after resampling.
+        ``return_token_timestamps`` as in ``generate``, with the clip's frame count (after resampling) as the attention
+        mask's."""
         self._require_engine()
+        n16 = (int(torch.as_tensor(pcm).numel()) if _rate(sampling_rate) == SAMPLE_RATE
+               else resampled_length(int(torch.as_tensor(pcm).numel()), _rate(sampling_rate), SAMPLE_RATE))
+        ts = (self._timestamp_request(None, task, self.pcm_num_frames(n16), time_precision)
+              if return_token_timestamps else None)
         if _rate(sampling_rate) != SAMPLE_RATE:
             x = torch.as_tensor(pcm).detach().to(torch.float32).reshape(-1)
             if resampled_length(x.numel(), _rate(sampling_rate), SAMPLE_RATE) > MAX_WINDOW_SAMPLES:
@@ -513,7 +581,8 @@ class WhisperMedusaModel:
             self._check_unsupported(temperature, None, kwargs)
             x16 = self._upload_16k(x, sampling_rate)
             self._encode_window(x16, Window(0, x16.numel(), 0, 0), torch.cuda.current_stream(self._device).cuda_stream)
-            return self._decode(language, task, kwargs, temperature, return_dict_in_generate=return_dict_in_generate)
+            return self._decode(language, task, kwargs, temperature, return_dict_in_generate=return_dict_in_generate,
+                                **({"token_timestamps": ts} if ts else {}))
         x = torch.as_tensor(pcm).detach().to("cpu", torch.float32).contiguous().reshape(-1)
         if x.numel() > 480000:
             raise NotImplementedError("Longform generation is not supported yet")
@@ -522,7 +591,8 @@ class WhisperMedusaModel:
                lib.wm_encode_pcm(self._handle, C.cast(x.data_ptr(), C.POINTER(C.c_float)), int(x.numel())),
                "wm_encode_pcm")
         self._check_unsupported(temperature, None, kwargs)
-        return self._decode(language, task, kwargs, temperature, return_dict_in_generate=return_dict_in_generate)
+        return self._decode(language, task, kwargs, temperature, return_dict_in_generate=return_dict_in_generate,
+                            **({"token_timestamps": ts} if ts else {}))
 
     # ------------------------------------------------------------------ long-form (HF chunked ASR pipeline)
     def transcribe(self, audio: Union[np.ndarray, torch.Tensor], sampling_rate: int = SAMPLE_RATE,
@@ -609,8 +679,9 @@ class WhisperMedusaModel:
                             avg_logprob=out.avg_logprob,
                             skipped=skip_window(out.no_speech_prob, out.avg_logprob, *no_speech))
 
-    def _decode(self, language, task, kwargs, temperature, generation_config=None,
-                return_dict_in_generate=None) -> Union[torch.Tensor, MedusaGenerateOutput]:
+    def _decode(self, language, task, kwargs, temperature, generation_config=None, return_dict_in_generate=None,
+                token_timestamps: Optional[Tuple[Optional[int], float]] = None) -> Union[torch.Tensor, MedusaGenerateOutput]:
+        """``token_timestamps``: ``(num_frames or None, time_precision)`` from ``_timestamp_request``, or None."""
         g = generation_config if generation_config is not None else self.generation_config
         output_scores = bool(kwargs.pop("output_scores", False))
         output_logits = bool(kwargs.pop("output_logits", False))
@@ -652,20 +723,102 @@ class WhisperMedusaModel:
         # engine after to() / close() starts with it off)
         ns_row = self._no_speech_row(prompt, g) if want_ns else -1
         _check(lib, self._handle, lib.wm_set_option(self._handle, b"no_speech_row", ns_row), "wm_set_option(no_speech_row)")
+        # alignment heads captured by this call's loop: sent on every call that asks for timestamps (a new engine after
+        # to() / close() starts with capture off), and switched off again on the engine that last had them
+        if token_timestamps is not None or getattr(self, "_ts_engine", None) == self._handle.value:
+            pairs = [int(v) for p in g.alignment_heads for v in p] if token_timestamps is not None else []
+            arr = (C.c_int32 * max(1, len(pairs)))(*pairs)
+            _check(lib, self._handle, lib.wm_set_alignment_heads(self._handle, arr, len(pairs) // 2),
+                   "wm_set_alignment_heads")
+            self._ts_engine = self._handle.value if pairs else None
         tr = self._run_loop(prompt, gp)
         self.last_trace = tr
         self._last_medusa_temperature = float(gp.temperature)
         out = self._strip(tr.sequences, len(prompt), int(gp.pad_token_id), int(gp.eos_token_id))
         sequences = torch.tensor([out], dtype=torch.long, device=self._device)
+        stamps = self._token_timestamps(tr, len(prompt), len(out), *token_timestamps) if token_timestamps else None
         if not as_dict:
+            if stamps is not None:     # the reference's {"sequences", "token_timestamps"} (model.py:1764-1769)
+                return MedusaGenerateOutput(sequences, None, None, None, None, None, token_timestamps=stamps)
             return sequences
         out = self._generate_output(sequences, tr, output_scores, output_logits)
+        out.token_timestamps = stamps
         if want_ns:
             prob = C.c_float(0.0)
             token = int(g.no_timestamps_token_id) - 1      # HF's choice (generation_whisper.py _setup_no_speech_detection)
             _check(lib, self._handle, lib.wm_last_no_speech(self._handle, token, C.byref(prob), None), "wm_last_no_speech")
             out.no_speech_prob = float(prob.value)
         return out
+
+    def _token_timestamps(self, tr: GenerateTrace, n_prompt: int, n_ids: int, num_frames: Optional[int],
+                          time_precision: float) -> torch.Tensor:
+        """HF's timestamps of the sequence up to and including its first EOS (``wm_token_timestamps``), cut to the
+        ``n_ids`` ids ``generate`` returns (the prompt and the trailing EOS stripped)."""
+        lib = _lib.load()
+        n_total = n_prompt + tr.n_new_tokens
+        buf = torch.zeros(max(1, n_total), dtype=torch.float32)
+        _check(lib, self._handle,
+               lib.wm_token_timestamps(self._handle, n_prompt, n_total, -1 if num_frames is None else int(num_frames),
+                                       int(getattr(self.config, "median_filter_width", 7)), float(time_precision),
+                                       C.cast(buf.data_ptr(), C.POINTER(C.c_float)), None, None), "wm_token_timestamps")
+        if n_ids > tr.n_new_tokens:
+            raise EngineError(f"{n_ids} ids returned for {tr.n_new_tokens} decoded tokens")
+        return buf[n_prompt : n_prompt + n_ids][None].to(self._device)
+
+    def last_alignment_probs(self, row0: int, n_rows: int) -> torch.Tensor:
+        """Cross-attention probabilities the last ``generate(..., return_token_timestamps=True)`` captured at positions
+        ``row0 .. row0 + n_rows - 1``: ``[alignment pairs, n_rows, 1500]`` (``wm_last_alignment_probs``)."""
+        self._require_engine()
+        lib = _lib.load()
+        n_pairs = C.c_int32(0)     # the pairs the engine captured with (the config may have changed since)
+        _check(lib, self._handle, lib.wm_last_alignment_probs(self._handle, 0, 0, None, 0, C.byref(n_pairs)),
+               "wm_last_alignment_probs")
+        out = torch.empty(n_pairs.value, int(n_rows), self.config.max_source_positions, dtype=torch.float32)
+        _check(lib, self._handle, lib.wm_last_alignment_probs(self._handle, int(row0), int(n_rows),
+                                                              C.cast(out.data_ptr(), C.POINTER(C.c_float)), out.numel(),
+                                                              None), "wm_last_alignment_probs")
+        return out
+
+    def timestamps_from_probs(self, probs: torch.Tensor, n_prompt: int, num_frames: Optional[int] = None,
+                              time_precision: float = 0.02, filter_width: Optional[int] = None):
+        """The extraction kernels on given probability rows ``probs [heads, N, W]`` (``wm_token_timestamps_from_probs``):
+        returns ``(timestamps [n_prompt + N + 1], matrix [N, F], jumps [N])``."""
+        self._require_engine()
+        lib = _lib.load()
+        p = torch.as_tensor(probs, dtype=torch.float32).detach().cpu().contiguous()
+        nh, n, w = (int(v) for v in p.shape)
+        f = w if num_frames is None else min(w, int(num_frames) // 2)
+        ts = torch.zeros(n_prompt + n + 1, dtype=torch.float32)
+        mat = torch.zeros(max(1, n * f), dtype=torch.float32)
+        jumps = torch.zeros(max(1, n), dtype=torch.int32)
+        width = int(filter_width if filter_width is not None else getattr(self.config, "median_filter_width", 7))
+        _check(lib, self._handle,
+               lib.wm_token_timestamps_from_probs(self._handle, C.cast(p.data_ptr(), C.POINTER(C.c_float)), nh, n, w,
+                                                  int(n_prompt), -1 if num_frames is None else int(num_frames), width,
+                                                  float(time_precision), C.cast(ts.data_ptr(), C.POINTER(C.c_float)),
+                                                  C.cast(mat.data_ptr(), C.POINTER(C.c_float)),
+                                                  C.cast(jumps.data_ptr(), C.POINTER(C.c_int32))),
+               "wm_token_timestamps_from_probs")
+        return ts, mat[: n * f].reshape(n, f), jumps[:n]
+
+    def last_timestamp_matrix(self, n_prompt: int, n_total: int, num_frames: Optional[int] = None,
+                              time_precision: float = 0.02):
+        """``(timestamps [n_total], matrix [N, F], jumps [N])`` of the last captured ``generate`` for its first
+        ``n_total`` ids (``wm_token_timestamps``), N = n_total - 1 - n_prompt."""
+        self._require_engine()
+        lib = _lib.load()
+        n = max(0, n_total - 1 - n_prompt)
+        f = self.config.max_source_positions if num_frames is None else min(self.config.max_source_positions,
+                                                                             int(num_frames) // 2)
+        ts = torch.zeros(max(1, n_total), dtype=torch.float32)
+        mat = torch.zeros(max(1, n * f), dtype=torch.float32)
+        jumps = torch.zeros(max(1, n), dtype=torch.int32)
+        _check(lib, self._handle,
+               lib.wm_token_timestamps(self._handle, int(n_prompt), int(n_total), -1 if num_frames is None else int(num_frames),
+                                       int(getattr(self.config, "median_filter_width", 7)), float(time_precision),
+                                       C.cast(ts.data_ptr(), C.POINTER(C.c_float)), C.cast(mat.data_ptr(), C.POINTER(C.c_float)),
+                                       C.cast(jumps.data_ptr(), C.POINTER(C.c_int32))), "wm_token_timestamps")
+        return ts[:n_total], mat[: n * f].reshape(n, f), jumps[:n]
 
     def _no_speech_row(self, prompt: Sequence[int], g) -> int:
         """Index in the prompt of the start-of-transcript token, whose raw base-head row gives the no-speech

@@ -149,6 +149,15 @@ class StreamGroup:
 
     def generate(self, input_features: torch.Tensor, **kwargs) -> List[torch.Tensor]:
         """``input_features [B, 80, 3000]`` with any B (the batch dimension the reference refuses, model.py:1451):
-        one result per row."""
-        rows = [input_features[i : i + 1] for i in range(input_features.shape[0])]
-        return self._run(rows, lambda m, x, kw: m.generate(x, **kw), kwargs)
+        one result per row.  ``attention_mask [B, 3000]`` (the feature extractor's): row i goes with clip i."""
+        B = input_features.shape[0]
+        mask = kwargs.pop("attention_mask", None)
+        if mask is not None:
+            mask = torch.as_tensor(mask)
+            if mask.dim() == 1:
+                mask = mask[None]
+            if mask.dim() != 2 or mask.shape[0] != B:
+                raise ValueError(f"attention_mask must have one row per clip, [{B}, 3000], got shape {tuple(mask.shape)}")
+        rows = [(input_features[i : i + 1], None if mask is None else mask[i : i + 1]) for i in range(B)]
+        return self._run(rows, lambda m, x, kw: m.generate(x[0], **kw) if x[1] is None else
+                         m.generate(x[0], attention_mask=x[1], **kw), kwargs)
