@@ -13,7 +13,13 @@ timestamps, so that a recording of any length transcribes as that pipeline would
 With ``no_speech_threshold`` and ``logprob_threshold``, a window is skipped by HF's no-speech rule (``skip_window``) and
 contributes no ids to the merge.
 
-The CPU tests pin both to the installed transformers; the package does not import it.
+Token timestamps (``transcribe(return_token_timestamps=True)``) restate what HF's ``tokenization_whisper._decode_asr``
+does with ``return_timestamps="word"`` for windows without timestamp tokens: ``window_offsets`` places each window on the
+recording's time axis, ``token_pairs`` turns its token times into ``(start, end)`` pairs, and ``merge_windows`` with
+``pairs`` is ``_find_longest_common_sequence(sequences, token_timestamp_sequences)``, whose match rule is stricter
+(equal ids whose times are in order), so its ids can differ from the untimed merge's.
+
+The CPU tests pin all of it to the installed transformers; the package does not import it.
 """
 from __future__ import annotations
 
@@ -76,32 +82,97 @@ def plan_windows(n_samples: int, chunk_len: int, stride_left: int, stride_right:
     return out
 
 
-def merge_windows(sequences: Sequence[Sequence[int]]) -> List[int]:
-    """Longest-common-sequence merge of the windows' ids, left to right (no windows: no ids)."""
+Pair = Tuple[float, float]
+
+
+def merge_windows(sequences: Sequence[Sequence[int]], pairs: Optional[Sequence[Sequence[Pair]]] = None):
+    """Longest-common-sequence merge of the windows' ids, left to right (no windows: no ids).
+
+    ``pairs``: one ``(start, end)`` per id of every window (``token_pairs``).  A position of the overlap then matches only
+    when the ids are equal and the left window's pair is ``<=`` the right window's (Python's tuple order, as HF compares
+    them), and the pairs are cut where the ids are; returns ``(ids, pairs)`` instead of ``ids``."""
+    timed = pairs is not None
     if len(sequences) == 0:
-        return []
+        return ([], []) if timed else []
     left = np.asarray(sequences[0], dtype=np.int64)
     total: List[int] = []
-    for right_seq in sequences[1:]:
+    if timed:
+        left_p = [tuple(p) for p in pairs[0]]
+        total_p: List[Pair] = []
+    for k, right_seq in enumerate(sequences[1:], start=1):
         right = np.asarray(right_seq, dtype=np.int64)
         n_l, n_r = len(left), len(right)
-        best = 0.0
+        # Shift i (1 <= i < n_l + n_r) lays the last i ids of the left window over the first ones of the right window:
+        # left[a] faces right[b] where b - a = i - n_l.  Its match count is the sum of that diagonal of the match matrix.
+        same = left[:, None] == right[None, :]
+        if timed:     # (ls, le) <= (rs, re) in tuple order
+            right_p = [tuple(p) for p in pairs[k]]
+            ls, le = (np.array([p[j] for p in left_p], dtype=np.float64).reshape(-1, 1) for j in (0, 1))
+            rs, re = (np.array([p[j] for p in right_p], dtype=np.float64).reshape(1, -1) for j in (0, 1))
+            same &= (ls < rs) | ((ls == rs) & (le <= re))
+        diag = (np.arange(n_r)[None, :] - np.arange(n_l)[:, None] + n_l - 1).ravel()       # = i - 1
+        matches = np.bincount(diag, weights=same.ravel(), minlength=max(0, n_l + n_r - 1)).astype(np.int64)
+        i = np.arange(1, n_l + n_r)
+        matching = matches / i + i / 10000.0       # the second term favours long perfect matches
+        matching[matches <= 1] = -np.inf
         best_idx = (n_l, n_l, 0, 0)
-        for i in range(1, n_l + n_r):
-            eps = i / 10000.0                      # favours long perfect matches
-            l0, l1 = max(0, n_l - i), min(n_l, n_l + n_r - i)
-            r0, r1 = max(0, i - n_l), min(n_r, i)
-            matches = int(np.count_nonzero(left[l0:l1] == right[r0:r1]))
-            matching = matches / i + eps
-            if matches > 1 and matching > best:
-                best = matching
-                best_idx = (l0, l1, r0, r1)
+        if len(i) and matching.max() > 0.0:        # the first shift of the largest score, as a strict left-to-right scan
+            i = int(i[int(np.argmax(matching))])
+            best_idx = (max(0, n_l - i), min(n_l, n_l + n_r - i), max(0, i - n_l), min(n_r, i))
         l0, l1, r0, r1 = best_idx
         # the left window is trusted for the first half of the overlap, the right window for the second
         total.extend(left[: (l0 + l1) // 2].tolist())
         left = right[(r0 + r1) // 2:]
+        if timed:
+            total_p.extend(left_p[: (l0 + l1) // 2])
+            left_p = right_p[(r0 + r1) // 2:]
     total.extend(left.tolist())
+    if timed:
+        total_p.extend(left_p)
+        return total, total_p
     return total
+
+
+def window_offsets(windows: Sequence) -> List[float]:
+    """Where each window starts on the recording's time axis, in seconds, as HF's ``_decode_asr`` accumulates it
+    (``window``: anything with ``start``, ``end``, ``stride_left`` and ``stride_right`` in 16 kHz samples).  The strides
+    are in seconds, as the pipeline's ``postprocess`` converts them; the offset drops by the left stride before a
+    window and grows by its length less its right stride after it, in the same order and in Python floats."""
+    offset, out = 0.0, []
+    for w in windows:
+        offset -= w.stride_left / SAMPLE_RATE
+        out.append(offset)
+        offset += (w.end - w.start) / SAMPLE_RATE - w.stride_right / SAMPLE_RATE
+    return out
+
+
+def token_pairs(ids: Sequence[int], times: Sequence[float], offset: float, eos_token_id: int) -> List[Pair]:
+    """``(start, end)`` in recording seconds of every text id of a window (``text_ids``' ids, in order), as HF's
+    ``_decode_asr`` forms them: ``start = round(times[i - 1] + offset, 2)`` (``round(0.0 + offset, 2)`` at ``i = 0``) and
+    ``end = round(times[i] + offset, 2)``.  ``ids`` and ``times`` are what ``generate(..., return_token_timestamps=True)``
+    returns for the window: HF's short-form ``sequences`` and ``token_timestamps`` carry no decoder prompt either, so
+    ``i`` indexes the same list here as there (the prompt's times are 0.0, so ``i = 0`` gives the same start either
+    way)."""
+    out: List[Pair] = []
+    for i, t in enumerate(ids):
+        if int(t) < eos_token_id:
+            start = round(0.0 + offset, 2) if i == 0 else round(float(times[i - 1]) + offset, 2)
+            out.append((start, round(float(times[i]) + offset, 2)))
+    return out
+
+
+def merge_timed(results: Sequence["WindowResult"], eos_token_id: int) -> Tuple[List[int], List[Pair]]:
+    """The timed merge of a transcription's windows (``WindowResult`` with ``token_timestamps``): every window is
+    placed by ``window_offsets``; a skipped window takes part as an empty one, as in the untimed merge."""
+    seqs, pairs = [], []
+    for r, offset in zip(results, window_offsets(results)):
+        if r.skipped:
+            seqs.append([])
+            pairs.append([])
+        else:
+            seqs.append(text_ids(r.ids, eos_token_id))
+            pairs.append(token_pairs(r.ids, r.token_timestamps.reshape(-1).tolist(), offset, eos_token_id))
+    return merge_windows(seqs, pairs)
 
 
 def text_ids(ids: Sequence[int], eos_token_id: int) -> List[int]:
@@ -148,7 +219,8 @@ class WindowResult:
     """One window of a long-form transcription (``WhisperMedusaModel.last_windows``)."""
 
     def __init__(self, window: Window, ids: List[int], trace, no_speech_prob: Optional[float] = None,
-                 avg_logprob: Optional[float] = None, skipped: Optional[bool] = None):
+                 avg_logprob: Optional[float] = None, skipped: Optional[bool] = None, token_timestamps=None,
+                 num_frames: Optional[int] = None):
         self.start, self.end = window.start, window.end
         self.stride_left, self.stride_right = window.stride_left, window.stride_right
         self.ids = ids            # what generate() returns for the window (prompt and trailing EOS stripped)
@@ -157,6 +229,9 @@ class WindowResult:
         self.no_speech_prob = no_speech_prob
         self.avg_logprob = avg_logprob
         self.skipped = skipped    # True: the window counts as silence and adds no ids to the merge
+        # transcribe(return_token_timestamps=True); both None without it
+        self.token_timestamps = token_timestamps   # FloatTensor[1, len(ids)], seconds from the window's start
+        self.num_frames = num_frames               # feature frames the alignment was cropped to
 
     def merge_ids(self, eos_token_id: int) -> List[int]:
         """What the window contributes to ``merge_windows``: its text ids, or none for a skipped window (its

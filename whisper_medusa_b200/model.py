@@ -32,8 +32,8 @@ import torch
 
 from . import _lib
 from .config import MedusaConfig, MedusaGenerationConfig
-from .longform import (MAX_WINDOW_SAMPLES, SAMPLE_RATE, Window, WindowResult, merge_windows, no_speech_rule,
-                       plan_windows, resampled_length, skip_window, window_params)
+from .longform import (MAX_WINDOW_SAMPLES, SAMPLE_RATE, Window, WindowResult, merge_timed, merge_windows,
+                       no_speech_rule, plan_windows, resampled_length, skip_window, window_params)
 from .weights import pack_blob
 
 N_FRAMES = 3000
@@ -124,7 +124,8 @@ class MedusaGenerateOutput:
     * ``token_timestamps`` (``return_token_timestamps=True``, else ``None``): ``FloatTensor[1, n]``, the time in seconds
       of every id of ``sequences[0]`` (HF ``_extract_token_timestamps``: DTW over the alignment heads' cross-attention),
       computed on the GPU (``csrc/timestamps.cu``).  Without ``return_dict_in_generate`` it is the only field besides
-      ``sequences``.
+      ``sequences``.  From ``transcribe(..., return_token_timestamps=True)`` it is ``FloatTensor[1, n, 2]``, the
+      ``(start, end)`` of every id in seconds of the recording, and the only field besides ``sequences``.
 
     Fields are attributes and keys (``out.scores`` / ``out["scores"]``); an integer indexes the fields that are not
     ``None``, in the order above, as HF ``ModelOutput`` does."""
@@ -599,7 +600,8 @@ class WhisperMedusaModel:
                    chunk_length_s: float = 30.0, stride_length_s: Optional[Union[float, Sequence[float]]] = None,
                    language: Optional[str] = None, task: Optional[str] = None, temperature=None,
                    no_speech_threshold: Optional[float] = None, logprob_threshold: Optional[float] = None,
-                   **generate_kwargs) -> torch.Tensor:
+                   return_token_timestamps: Optional[bool] = None, time_precision: float = 0.02,
+                   **generate_kwargs) -> Union[torch.Tensor, MedusaGenerateOutput]:
         """Transcribe a mono recording of any length at any integer sampling rate; returns ``LongTensor[1, n]``.
 
         The semantics of HF's ``pipeline("automatic-speech-recognition", chunk_length_s=30)`` without timestamps
@@ -618,21 +620,44 @@ class WhisperMedusaModel:
         the merge -- when the probability of ``<|nospeech|>`` at its start-of-transcript position is above
         ``no_speech_threshold`` and the average log-probability of its tokens is below ``logprob_threshold``.  Each
         window is still decoded in full (the rule needs its average log-probability).  ``no_speech_threshold`` alone
-        raises ``ValueError``; ``logprob_threshold`` alone (temperature fallback) ``NotImplementedError``."""
+        raises ``ValueError``; ``logprob_threshold`` alone (temperature fallback) ``NotImplementedError``.
+
+        ``return_token_timestamps=True``: a ``MedusaGenerateOutput`` whose ``sequences`` (``LongTensor[1, n]``) and
+        ``token_timestamps`` (``FloatTensor[1, n, 2]``, the ``(start, end)`` of every id in seconds of the recording) are
+        what HF's pipeline gives with ``return_timestamps="word"`` for windows without timestamp tokens
+        (``_decode_asr``).  Each window is decoded as ``generate_from_pcm(window, return_token_timestamps=True,
+        time_precision=...)`` would decode it, cropped to its own frames; its times are moved by the window's offset and
+        the windows are merged by HF's timed rule, which matches overlapping ids only when their times are in order.
+        The merged ids can therefore differ from those of the call without timestamps.  ``last_windows[i]`` holds each
+        window's ``token_timestamps`` (relative to the window) and ``num_frames``.  The checks of ``generate``'s flag
+        (``alignment_heads``, filter width, a chain of ``medusa_choices``) run before anything is uploaded."""
         self._require_engine()
         params = window_params(chunk_length_s, stride_length_s)
         _check_recording(audio, sampling_rate)
         no_speech = ((float(no_speech_threshold), float(logprob_threshold))
                      if no_speech_rule(no_speech_threshold, logprob_threshold) else None)
         self._check_unsupported(temperature, None, generate_kwargs)
+        if return_token_timestamps:
+            self._timestamp_request(None, task, None, time_precision)
+            generate_kwargs["time_precision"] = float(time_precision)
         x16 = self._upload_16k(audio, sampling_rate)
         stream = torch.cuda.current_stream(self._device).cuda_stream
         results = [self._transcribe_window(x16, w, stream, language=language, task=task, temperature=temperature,
                                            no_speech=no_speech, **generate_kwargs)
                    for w in plan_windows(x16.numel(), *params)]
         self.last_windows = results
-        merged = merge_windows([r.merge_ids(int(self.generation_config.eos_token_id)) for r in results])
-        return torch.tensor([merged], dtype=torch.long, device=self._device)
+        return self._merge_results(results, bool(return_token_timestamps))
+
+    def _merge_results(self, results: List[WindowResult], timed: bool) -> Union[torch.Tensor, MedusaGenerateOutput]:
+        """The windows' merge: ``LongTensor[1, n]``, or with token timestamps the output of ``transcribe``."""
+        eos = int(self.generation_config.eos_token_id)
+        if not timed:
+            merged = merge_windows([r.merge_ids(eos) for r in results])
+            return torch.tensor([merged], dtype=torch.long, device=self._device)
+        ids, pairs = merge_timed(results, eos)
+        return MedusaGenerateOutput(torch.tensor([ids], dtype=torch.long, device=self._device), None, None, None, None,
+                                    None, token_timestamps=torch.tensor(pairs, dtype=torch.float32).reshape(1, -1, 2)
+                                    .to(self._device))
 
     def _upload_16k(self, audio, sampling_rate) -> torch.Tensor:
         """The recording as contiguous f32 16 kHz samples on the engine's device: one upload (none for a CUDA tensor on
@@ -667,17 +692,25 @@ class WhisperMedusaModel:
                "wm_encode_pcm_device")
 
     def _transcribe_window(self, x16: torch.Tensor, w: Window, producer_stream: int, language=None, task=None,
-                           temperature=None, no_speech: Optional[Tuple[float, float]] = None, **kwargs) -> WindowResult:
-        """One window; ``no_speech`` = (no_speech_threshold, logprob_threshold) or None (the rule off)."""
+                           temperature=None, no_speech: Optional[Tuple[float, float]] = None,
+                           time_precision: Optional[float] = None, **kwargs) -> WindowResult:
+        """One window; ``no_speech`` = (no_speech_threshold, logprob_threshold) or None (the rule off);
+        ``time_precision`` = token timestamps with that precision, cropped to the window's frames, or None (off)."""
         self._encode_window(x16, w, producer_stream)
+        num_frames = None if time_precision is None else self.pcm_num_frames(w.end - w.start)
+        ts = {} if time_precision is None else {"token_timestamps": (num_frames, float(time_precision))}
         if no_speech is None:
-            ids = self._decode(language, task, kwargs, temperature)[0].tolist()
-            return WindowResult(w, ids, self.last_trace)
+            out = self._decode(language, task, kwargs, temperature, **ts)
+            if not ts:
+                return WindowResult(w, out[0].tolist(), self.last_trace)
+            return WindowResult(w, out.sequences[0].tolist(), self.last_trace, token_timestamps=out.token_timestamps,
+                                num_frames=num_frames)
         out = self._decode(language, task, dict(kwargs, output_no_speech_prob=True), temperature,
-                           return_dict_in_generate=True)
+                           return_dict_in_generate=True, **ts)
         return WindowResult(w, out.sequences[0].tolist(), self.last_trace, no_speech_prob=out.no_speech_prob,
                             avg_logprob=out.avg_logprob,
-                            skipped=skip_window(out.no_speech_prob, out.avg_logprob, *no_speech))
+                            skipped=skip_window(out.no_speech_prob, out.avg_logprob, *no_speech),
+                            token_timestamps=out.token_timestamps, num_frames=num_frames)
 
     def _decode(self, language, task, kwargs, temperature, generation_config=None, return_dict_in_generate=None,
                 token_timestamps: Optional[Tuple[Optional[int], float]] = None) -> Union[torch.Tensor, MedusaGenerateOutput]:

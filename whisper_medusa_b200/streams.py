@@ -120,9 +120,9 @@ class StreamGroup:
         Each recording is uploaded and resampled once into a device buffer that every engine reads; the windows of all
         recordings go into one work queue, so they decode concurrently on the S engines, and each recording's windows
         are merged in order.  The results equal ``model.transcribe`` of each recording, with the same
-        ``no_speech_threshold`` / ``logprob_threshold`` rule.  Per-window results:
-        ``self.last_windows[i]`` for recording i."""
-        from .longform import merge_windows, no_speech_rule, plan_windows, window_params
+        ``no_speech_threshold`` / ``logprob_threshold`` rule and ``return_token_timestamps`` / ``time_precision`` (then
+        one ``MedusaGenerateOutput`` per recording).  Per-window results: ``self.last_windows[i]`` for recording i."""
+        from .longform import no_speech_rule, plan_windows, window_params
         from .model import _check_recording
 
         recs = [recordings] if isinstance(recordings, (np.ndarray, torch.Tensor)) else list(recordings)
@@ -135,17 +135,20 @@ class StreamGroup:
         nst, lpt = kwargs.pop("no_speech_threshold", None), kwargs.pop("logprob_threshold", None)
         if no_speech_rule(nst, lpt):     # (same rule and arguments as model.transcribe)
             kwargs["no_speech"] = (float(nst), float(lpt))
+        timed = bool(kwargs.pop("return_token_timestamps", None))
+        time_precision = kwargs.pop("time_precision", 0.02)
         lead = self.models[0]
         lead._check_unsupported(kwargs.get("temperature"), None,
                                 {k: v for k, v in kwargs.items() if k not in ("language", "task", "temperature", "no_speech")})
+        if timed:
+            lead._timestamp_request(None, kwargs.get("task"), None, time_precision)
+            kwargs["time_precision"] = float(time_precision)
         x16 = [lead._upload_16k(r, sr) for r, sr in zip(recs, rates)]
         stream = torch.cuda.current_stream(self.device).cuda_stream     # every window's encode is ordered after it
         items = [(i, w) for i, x in enumerate(x16) for w in plan_windows(x.numel(), *params)]
         results = self._run(items, lambda m, it, kw: m._transcribe_window(x16[it[0]], it[1], stream, **kw), kwargs)
-        eos = int(lead.generation_config.eos_token_id)
         self.last_windows = [[res for (i, _), res in zip(items, results) if i == k] for k in range(len(recs))]
-        return [torch.tensor([merge_windows([r.merge_ids(eos) for r in ws])], dtype=torch.long, device=self.device)
-                for ws in self.last_windows]
+        return [lead._merge_results(ws, timed) for ws in self.last_windows]
 
     def generate(self, input_features: torch.Tensor, **kwargs) -> List[torch.Tensor]:
         """``input_features [B, 80, 3000]`` with any B (the batch dimension the reference refuses, model.py:1451):
