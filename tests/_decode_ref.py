@@ -58,7 +58,8 @@ def check_error(err, bar, case, what, oracle_fp32_err=None):
 def decode_logits(cfg, sd, enc, kw, n_iters, dtype=torch.float64, threads=16, prompt=None, begin_index=None,
                   prompt_len=None, tree_attention=False):
     """Oracle decode loop (engine regime, working dtype ``dtype``) started from the given encoder states; the trace
-    holds the raw pass-A / pass-B logits of the first ``n_iters`` iterations.
+    holds the raw pass-A / pass-B logits of the first ``n_iters`` iterations.  ``sd`` may also be a ``RefWeights``
+    already in the working dtype (``dtype`` is then ignored): at large-v2 a conversion costs seconds and 12 GB in fp64.
 
     ``prompt``: decoder ids to start from (default: the model's start tokens).  Given an engine's history up to the start
     of iteration n together with ``begin_index`` / ``prompt_len`` of the ORIGINAL prompt (so that the begin-suppress and
@@ -66,7 +67,7 @@ def decode_logits(cfg, sd, enc, kw, n_iters, dtype=torch.float64, threads=16, pr
     tokens of iteration n of the real run: pass A recomputes every cached row from the ids alone, which for chains and
     for ``tree_attention=True`` is what the real loop's cache holds (tests/test_oracle_history_prompt.py)."""
     torch.set_num_threads(threads)
-    w = W.RefWeights(sd, dtype)
+    w = sd if isinstance(sd, W.RefWeights) else W.RefWeights(sd, dtype)
     if prompt is None:
         prompt = M.init_tokens(cfg, kw.get("language"))
     extra = {k: kw[k] for k in ("posterior_alpha", "posterior_threshold") if k in kw}
@@ -81,8 +82,9 @@ def decode_logits(cfg, sd, enc, kw, n_iters, dtype=torch.float64, threads=16, pr
 
 
 def forward_logits(cfg, sd, enc, ids, dtype=torch.float64):
-    """Oracle of ``forward(decoder_input_ids=[ids])``: stacked head logits ``[K+1, T, V]`` from an empty cache."""
-    w = W.RefWeights(sd, dtype)
+    """Oracle of ``forward(decoder_input_ids=[ids])``: stacked head logits ``[K+1, T, V]`` from an empty cache (``sd``: a
+    state dict or a ``RefWeights``, as in ``decode_logits``)."""
+    w = sd if isinstance(sd, W.RefWeights) else W.RefWeights(sd, dtype)
     cache = W.new_cache(cfg)
     hidden = W.decoder_forward(w, cfg, list(ids), list(range(len(ids))), enc, cache, "engine")
     return W.medusa_logits(w, cfg, hidden, enc, cache, False, "engine")

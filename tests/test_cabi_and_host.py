@@ -103,6 +103,19 @@ def test_weight_layout_and_packing(engine_lib, preset, htype):
         engine_lib.wm_destroy(h)
 
 
+def test_create_takes_39_decoder_layers_and_a_block_layer_but_not_40_layers(engine_lib):
+    """The per-layer tables hold 40 decoder layers (WM_MAX_DEC_LAYERS): 39 layers plus the Medusa-Block layer fill them;
+    40 layers leave no record for a Block layer and are rejected for either head type."""
+    for htype in ("base_head", "medusa_block"):
+        h = _layout_handle(engine_lib, preset_config("micro", heads=4, heads_type=htype, decoder_layers=39))
+        engine_lib.wm_destroy(h)
+        wc = WhisperMedusaModel(preset_config("micro", heads=4, heads_type=htype, decoder_layers=40), None)._wm_config()
+        h = C.c_void_p()
+        assert engine_lib.wm_create(C.byref(wc), -1, C.byref(h)) == -1, htype
+        assert b"decoder layers" in engine_lib.wm_last_error(h)
+        engine_lib.wm_destroy(h)
+
+
 def test_create_rejects_unsupported_shapes(engine_lib):
     cfg = preset_config("micro", heads=4)
     m = WhisperMedusaModel(cfg, None)

@@ -5,7 +5,8 @@ import pytest
 import torch
 
 from oracle import whisper_ref as W
-from whisper_medusa_b200.synthetic import ENCODER_PROFILES, synthetic_audio, synthetic_state_dict, width_config
+from whisper_medusa_b200.synthetic import (ENCODER_PROFILES, preset_config, synthetic_audio, synthetic_state_dict,
+                                           width_config)
 
 ENC = "whisper_model.model.encoder"
 
@@ -121,6 +122,57 @@ def test_encoder_profiles_reach_their_regime(profile, d):
             assert st["spread"] > 30
         elif profile == "near_top":
             assert min(points["q"], points["v"], points["fc1"]) > 1e4 and max(points.values()) < 3.5e4
+
+
+@pytest.mark.parametrize("profile", ENCODER_PROFILES)
+def test_encoder_profiles_at_full_depth(profile):
+    """Each encoder profile in every one of medium's 24 layers on 30 s of audio (DESIGN.md section 2, "Profiles at
+    depth"): every fp16 rounding point below 65504 (measured at most 2.0e4, near_top) and each profile in its regime in
+    every layer, except ``small``, whose eps-dominated rows occur in the first layers only (the residual grows with
+    depth: the smallest row std per layer is 1.4e-3 to 1.5e-2)."""
+    cfg = preset_config("medium", heads=4)
+    sd = synthetic_state_dict(cfg, seed=1, encoder_profile=profile)
+    w = W.RefWeights(sd, torch.float64)
+    per = {}
+
+    def probe(name, t):
+        if not name.startswith("layers."):
+            return
+        _, layer, key = name.split(".")
+        st = per.setdefault(int(layer), {"mu_sigma": 0.0, "std_min": float("inf"), "outlier": 0.0, "spread": 0.0})
+        if key.endswith("_in"):
+            mu, sg = t.mean(-1), t.std(-1, unbiased=False)
+            a = t.abs()
+            st["mu_sigma"] = max(st["mu_sigma"], float((mu.abs() / sg).max()))
+            st["std_min"] = min(st["std_min"], float(sg.min()))
+            st["outlier"] = max(st["outlier"], float((a.max(-1).values / a.median(-1).values).max()))
+        elif key == "scores":
+            st["spread"] = max(st["spread"], float((t.max(-1).values - t.min(-1).values).max()))
+        else:
+            st[key] = max(st.get(key, 0.0), float(t.abs().max()) * (64 ** 0.5 if key == "q" else 1.0))
+
+    w.enc_probe = probe
+    mel = torch.from_numpy(W.log_mel_spectrogram(synthetic_audio(30.0, stream_id=1), torch.float64))
+    assert torch.isfinite(W.encoder_forward(w, cfg, mel, "engine")).all()
+    w.enc_probe = None       # the probe refers to w: without this cycle the weights are freed at once
+    assert sorted(per) == list(range(cfg.encoder_layers))
+    for i, st in per.items():
+        points = {k: st[k] for k in ("ln1", "q", "k", "v", "attn", "ln2", "fc1")}
+        where = (profile, i, st)
+        assert max(points.values()) < 65504.0, where
+        if profile == "default":
+            assert st["mu_sigma"] < 2 and st["std_min"] > 0.3 and st["outlier"] < 20 and st["spread"] < 15, where
+            assert max(points.values()) < 10, where
+        elif profile == "offset":
+            assert st["mu_sigma"] > 50, where
+        elif profile == "outliers":
+            assert st["outlier"] > 100, where
+        elif profile == "small":
+            assert st["std_min"] < 0.02 and (i > 0 or st["std_min"] ** 2 < 1e-5), where
+        elif profile == "peaked":
+            assert st["spread"] > 10, where
+        elif profile == "near_top":
+            assert min(points["q"], points["v"], points["fc1"]) > 1e4 and max(points.values()) < 3.5e4, where
 
 
 def test_encoder_and_decoder_profiles_are_independent():

@@ -32,6 +32,22 @@ def test_default_state_dict_is_unchanged(preset, heads, htype, seed, digest):
     assert _digest(synthetic_state_dict(cfg, seed=seed, encoder_profile="default")) == digest
 
 
+def test_whisper_size_presets():
+    """OpenAI's published dimensions of the multilingual sizes; each shares large-v2's vocabulary and special tokens."""
+    large = preset_config("large-v2")
+    dims = {"base": (512, 8, 6, 2048), "small": (768, 12, 12, 3072), "medium": (1024, 16, 24, 4096),
+            "large-v2": (1280, 20, 32, 5120)}
+    for name, (d, h, layers, ffn) in dims.items():
+        cfg = preset_config(name, heads=4)
+        assert (cfg.d_model, cfg.medusa_hidden_size, cfg.encoder_attention_heads, cfg.decoder_attention_heads) == (d, d, h, h)
+        assert (cfg.encoder_layers, cfg.decoder_layers, cfg.encoder_ffn_dim, cfg.decoder_ffn_dim) == (layers, layers, ffn, ffn)
+        assert cfg.max_source_positions == 1500 and cfg.max_target_positions == 448 and cfg.is_multilingual
+        for k in ("vocab_size", "eos_token_id", "decoder_start_token_id", "no_timestamps_token_id", "suppress_tokens",
+                  "begin_suppress_tokens", "lang_to_id", "task_to_id"):
+            assert getattr(cfg, k) == getattr(large, k), (name, k)
+    assert large.vocab_size == 51865
+
+
 def test_width_config_and_d_model_override():
     for d in (128, 256, 512, 640, 768, 1024, 1280):
         cfg = width_config(d)
@@ -46,25 +62,31 @@ def test_width_config_and_d_model_override():
     assert tuple(sd["medusa_heads.0.0.linear.weight"].shape) == (256, 256)
 
 
-def _decode_fp64_with_probe(cfg, sd, enc):
-    """Runs a 5-token decoder pass + Medusa heads in fp64; returns (logits, per-LayerNorm-input statistics)."""
-    w = W.RefWeights(sd, torch.float64)
+def _decode_fp64_with_probe(cfg, sd, enc, per_layer=None):
+    """Runs a 5-token decoder pass + Medusa heads in fp64; returns (logits, per-LayerNorm-input statistics).  Given a
+    dict ``per_layer``, it also collects the statistics of each decoder layer's three folded LayerNorms separately.
+    The encoder's tensors are not converted (``enc`` is given): at large-v2 they are 5 GB in fp64."""
+    w = W.RefWeights({k: v for k, v in sd.items() if not k.startswith("whisper_model.model.encoder.")}, torch.float64)
     stats = {"mu_sigma": [], "gx": [], "outlier": []}
 
     def probe(prefix, x):
         if not prefix.endswith("layer_norm") or prefix.endswith("decoder.layer_norm"):
             return
         mu, sig = x.mean(-1), x.std(-1, unbiased=False)
-        stats["mu_sigma"].append(mu.abs() / sig)
-        stats["gx"].append((x * w[prefix + ".weight"]).abs())
         a = x.abs()
-        stats["outlier"].append(a.max(-1).values / a.median(-1).values)
+        st = {"mu_sigma": mu.abs() / sig, "gx": (x * w[prefix + ".weight"]).abs(),
+              "outlier": a.max(-1).values / a.median(-1).values}
+        for k, v in st.items():
+            stats[k].append(v)
+            if per_layer is not None:
+                per_layer.setdefault(prefix.split(".layers.")[-1].split(".")[0], {}).setdefault(k, []).append(v)
 
     w.ln_probe = probe
     cache = W.new_cache(cfg)
     ids = [cfg.decoder_start_token_id, cfg.no_timestamps_token_id, 17, 33, 64]
     hidden = W.decoder_forward(w, cfg, ids, list(range(len(ids))), enc, cache, "engine")
     logits = W.medusa_logits(w, cfg, hidden, enc, cache, False, "engine")
+    w.ln_probe = None        # the probe refers to w: without this cycle the weights are freed at once
     return logits, {k: torch.cat([t.reshape(-1) for t in v]) for k, v in stats.items()}
 
 
@@ -96,6 +118,44 @@ def test_activation_profiles_reach_their_regime(profile, d):
         assert float(gx.median()) < 0.125 and float(gx.max()) < 1.0       # fp16 lo half subnormal below ~0.125
     elif profile == "near_top":
         assert float(gx.max()) > 2e4
+
+
+@pytest.mark.parametrize("preset", ["medium", "large-v2"])
+@pytest.mark.parametrize("profile", ACTIVATION_PROFILES)
+def test_activation_profiles_at_full_depth(profile, preset):
+    """Each profile at 24 and 32 layers, per decoder layer (DESIGN.md section 2, "Profiles at depth"): |mean| / std at
+    every LayerNorm input, the largest |gamma o x| over the three folded LayerNorms and the share of gamma o x below
+    0.125 (where the fp16 lo half of the split is subnormal).  Every layer stays inside the operand window
+    (|gamma o x| < 65504, measured at most 3.0e4 under near_top).  The residual stream grows with depth, so the
+    2-layer bounds that scale with it are widened: default reaches |gamma o x| 124 at 32 layers, and under ``small``
+    the share below 0.125 falls from over 0.9 in layer 0 to about 0.2 in the deepest layers (the profile's regime is its first
+    layers; deeper ones are ordinary small activations, still far from the window's top)."""
+    cfg = preset_config(preset, heads=4)
+    sd = synthetic_state_dict(cfg, seed=1, activation_profile=profile)
+    enc = torch.randn(1500, cfg.d_model, generator=torch.Generator().manual_seed(0), dtype=torch.float64)
+    layers = {}
+    logits, _ = _decode_fp64_with_probe(cfg, sd, enc, layers)
+    assert torch.isfinite(logits).all() and float(logits.std()) > 0.5
+    assert sorted(layers, key=int) == [str(i) for i in range(cfg.decoder_layers)]
+    for i in range(cfg.decoder_layers):
+        st = {k: torch.cat([t.reshape(-1) for t in v]) for k, v in layers[str(i)].items()}
+        ms, gx, outl = float(st["mu_sigma"].max()), st["gx"], float(st["outlier"].max())
+        low = float((gx < 0.125).double().mean())
+        where = (preset, profile, i, ms, float(gx.max()), low, outl)
+        assert float(gx.max()) < 65504.0, where
+        if profile in ("default", "gamma_spread"):
+            assert ms < 0.2 and outl < 20, where
+            assert float(gx.max()) < (200.0 if profile == "default" else 1000.0), where
+        elif profile == "offset":
+            assert 5 < ms < 600 and float(gx.max()) < 1000.0, where
+        elif profile == "outliers":
+            assert outl > 50, where
+        elif profile == "small":
+            assert low > 0.15 and float(gx.max()) < 4.0, where
+        elif profile == "near_top":
+            assert float(gx.max()) > 2e4, where
+        if i == 0 and profile == "small":
+            assert low > 0.9, where
 
 
 @pytest.mark.parametrize("preset,htype,seed", [("micro", "base_head", 0), ("micro", "medusa_block", 1),

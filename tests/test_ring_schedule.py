@@ -34,8 +34,22 @@ def test_block_heads_and_16_node_trees(engine_lib, d, grid):
     _check(engine_lib, d, grid, K=3, n_tree=16)
 
 
+#: (d_model, decoder layers, Block layer): every Whisper size at its real depth, and the deepest model wm_create takes
+#: (39 layers + the Block layer = all 40 decoder-layer records)
+DEPTHS = ((384, 4, 0), (512, 6, 0), (768, 12, 0), (1024, 24, 0), (1280, 32, 0), (128, 39, 0), (128, 39, 1))
+
+
+@pytest.mark.parametrize("d,n_layers,block", DEPTHS, ids=[f"d{d}-L{n}" + ("-block" if b else "") for d, n, b in DEPTHS])
+def test_schedule_at_full_depth(engine_lib, d, n_layers, block):
+    """The stage records and weight chunks of every layer, not just layers 0 and 1: a chain with K = 10 on the full grid
+    and a 16-node tree with K = 3 on 37 CTAs."""
+    _check(engine_lib, d, 132, block=block, n_layers=n_layers)
+    _check(engine_lib, d, 37, block=block, K=3, n_tree=16, n_layers=n_layers)
+
+
 def test_rejects_out_of_range_shapes(engine_lib):
     bad = C.c_int32(-1)
     first = (C.c_int32 * 4)()
-    for args in [(100, 2, 0, 10, 11, 132), (512, 0, 0, 10, 11, 132), (512, 2, 0, 10, 17, 132), (512, 2, 0, 10, 11, 0)]:
+    for args in [(100, 2, 0, 10, 11, 132), (512, 0, 0, 10, 11, 132), (512, 2, 0, 10, 17, 132), (512, 2, 0, 10, 11, 0),
+                 (128, 40, 0, 10, 11, 132), (128, 40, 1, 10, 11, 132)]:
         assert engine_lib.wm_ring_schedule_check(*args, C.byref(bad), first) != 0, args

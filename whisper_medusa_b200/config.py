@@ -117,6 +117,13 @@ WHISPER_PRESETS: Dict[str, Dict[str, Any]] = {
         lang_to_id={}, task_to_id={}, no_timestamps_token_id=502, max_length=448,
     ),
 }
+# The multilingual sizes between tiny and large (OpenAI's published dimensions: d_model, heads, encoder = decoder
+# layers, FFN width) share large-v2's vocabulary, special tokens and suppress lists.
+for _name, (_d, _h, _l, _f) in {"openai/whisper-base": (512, 8, 6, 2048), "openai/whisper-small": (768, 12, 12, 3072),
+                                "openai/whisper-medium": (1024, 16, 24, 4096)}.items():
+    WHISPER_PRESETS[_name] = dict(copy.deepcopy(WHISPER_PRESETS["openai/whisper-large-v2"]), d_model=_d,
+                                  encoder_layers=_l, encoder_attention_heads=_h, encoder_ffn_dim=_f,
+                                  decoder_layers=_l, decoder_attention_heads=_h, decoder_ffn_dim=_f)
 
 _GENERATION_KEYS = (
     "suppress_tokens", "begin_suppress_tokens", "lang_to_id", "task_to_id",

@@ -344,11 +344,15 @@ def synthetic_audio(seconds: float, stream_id: int = 0, seed: int = 1234) -> np.
 
 
 def preset_config(name: str, heads: int = 10, heads_type: str = "base_head", **kw) -> MedusaConfig:
-    """BASELINE.json configs: ``large-v2`` (cfg 2-5), ``tiny.en`` (cfg 1), ``micro`` (tests)."""
+    """BASELINE.json configs: ``large-v2`` (cfg 2-5), ``tiny.en`` (cfg 1), ``micro`` (tests); ``base``, ``small`` and
+    ``medium`` (the full-depth tests)."""
     table = {
         "large-v2": "openai/whisper-large-v2",
         "tiny.en": "openai/whisper-tiny.en",
         "micro": "synthetic/whisper-micro",
+        "base": "openai/whisper-base",
+        "small": "openai/whisper-small",
+        "medium": "openai/whisper-medium",
     }
     wname = table.get(name, name)
     from .config import WHISPER_PRESETS
