@@ -241,6 +241,12 @@ int wm_enc_gemm_tile(int32_t M, int32_t N, int32_t K, int32_t fp16_out, int32_t 
  * L, need_a, cta} of the first of them. */
 int wm_ring_schedule_check(int32_t d_model, int32_t n_layers, int32_t medusa_block, int32_t K, int32_t n_tree,
                            int32_t n_cta, int32_t* n_bad, int32_t* first4);
+/* The same replay with the producer's L2 prefetch cursor at l2_budget bytes per CTA (0, or at least one 41,984-byte
+ * chunk; the build's own budget is WM_RING_L2_AHEAD, which wm_ring_schedule_check uses): every prefetched row is copied
+ * later in the launch in prefetch order or is one of the first rows of the tail program, the bytes prefetched and not
+ * yet copied never exceed the budget, and with a budget every copy was prefetched first. */
+int wm_ring_prefetch_check(int32_t d_model, int32_t n_layers, int32_t medusa_block, int32_t K, int32_t n_tree,
+                           int32_t n_cta, int32_t l2_budget, int32_t* n_bad, int32_t* first4);
 /* Debug: per-stage timeline of the last persistent iteration (after wm_set_option(h, "profile", 1)).
  * Rows of 24 int64: stage id, mode, layer; body ns and barrier-wait ns seen by the last CTA; then the
  * 16 raw probes of CTA 0 -- ns offsets from stage begin ([1] end of body, [2] end of barrier, [7] record

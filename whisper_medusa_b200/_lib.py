@@ -80,6 +80,8 @@ SYMBOLS = {
     "wm_enc_gemm_tile": (C.c_int, [C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, _P(C.c_int32)]),
     "wm_ring_schedule_check": (C.c_int, [C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                          _P(C.c_int32), _P(C.c_int32)]),
+    "wm_ring_prefetch_check": (C.c_int, [C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                                         _P(C.c_int32), _P(C.c_int32)]),
     "wm_set_option": (C.c_int, [C.c_void_p, C.c_char_p, C.c_int32]),
     "wm_get_stage_profile": (C.c_int, [C.c_void_p, _P(C.c_int64), C.c_int32, _P(C.c_int32)]),
 }

@@ -43,6 +43,9 @@ struct ChunkDesc {
   uint16_t sa_item;
   uint8_t sa_mode, sa_block;
 };
+// The largest ring slot of any width (RingGeom<1280>::SLOT_BYTES: 16 rows of the 1280 x 2 + 64-byte ring row stride),
+// so no chunk is larger.  A nonzero L2 lookahead of the ring producer must hold at least this much.
+#define WM_RING_SLOT_MAX (16 * (1280 * 2 + 64))
 
 // One stage of the persistent ring kernel, fully resolved for one CTA by the host (built once per
 // model, [instruction][cta], 128 B each): the kernel never derives shapes, row ranges or pointers on

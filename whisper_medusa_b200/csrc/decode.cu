@@ -1759,12 +1759,17 @@ void dec_build_ring_tables(const DecModel& hm, const float2* ln_fold, int ncta, 
 }
 
 // Host replay of the ring protocol (no GPU): for each CTA and each launch state, the chunks the producer warp copies
-// (ring_producer) against what the compute warps expect in the slots they take (stage_gemm_ring, stage_cross_attn_ring,
-// stage_self_attn_ring), compared as (source, rows, bytes).  Launch states: every kv0 in [0, WM_MAX_POS - 16] with sweep A
-// skipped (L0 = kv0), with sweep A over t_a = 1 ... 16 rows (L0 = kv0 + t_a), and prefill chunks of 16 rows; those whose
-// verify rows would pass WM_MAX_POS are left out.  Returns the number of (launch, CTA) pairs whose sequences differ;
-// `first` receives {kv0, L0, need_a, cta} of the first of them.
-int dec_check_ring_schedule(const DecModel& hm, int ncta, int first[4]) {
+// (ring_walk, as ring_producer runs it) against what the compute warps expect in the slots they take (stage_gemm_ring,
+// stage_cross_attn_ring, stage_self_attn_ring), compared as (source, rows, bytes).  The walk's L2 prefetches at
+// `budget` bytes (< 0: the built WM_RING_L2_AHEAD) are replayed along, chunk by chunk: each must be copied later in the
+// same launch, in prefetch order, or be one of the first weight chunks of the tail program (the next launch's); the
+// bytes prefetched and not yet copied never exceed the budget; and with a budget every copy was prefetched first.
+// Launch states: every kv0 in [0, WM_MAX_POS - 16] with sweep A skipped (L0 = kv0), with sweep A over t_a = 1 ... 16
+// rows (L0 = kv0 + t_a), and prefill chunks of 16 rows; those whose verify rows would pass WM_MAX_POS are left out.
+// Returns the number of (launch, CTA) pairs whose sequences differ or whose prefetches break a rule; `first` receives
+// {kv0, L0, need_a, cta} of the first of them.
+int dec_check_ring_schedule(const DecModel& hm, int ncta, long long budget, int first[4]) {
+  const uint32_t l2_ahead = budget < 0 ? (uint32_t)WM_RING_L2_AHEAD : (uint32_t)budget;
   std::vector<CtaStage> stab;
   std::vector<ChunkDesc> ctab;
   std::vector<int> off;
@@ -1805,18 +1810,43 @@ int dec_check_ring_schedule(const DecModel& hm, int ncta, int first[4]) {
     }
   }
   std::vector<Copy> prod, cons;
+  // prefetched chunks not yet matched by a copy, in prefetch order: [pf_head, pending.size())
+  std::vector<ChunkCopy> pending;
+  auto same = [](const ChunkCopy& x, const ChunkCopy& y) {
+    return x.src == y.src && x.row_bytes == y.row_bytes && x.nrows == y.nrows && x.copy_bytes == y.copy_bytes;
+  };
   int bad = 0;
   auto run = [&](int L0, int kv0, int need_a, int prefill) {
     for (int cta = 0; cta < ncta; ++cta) {
       prod.clear();
       cons.clear();
+      pending.clear();
+      size_t pf_head = 0;
       const int* o = &off[(size_t)cta * 4];
-      for (int c = need_a ? o[0] : o[1]; c < (prefill ? o[1] : o[3]); ++c) {
-        const ChunkDesc& dsc = ctab[c];
-        if (dsc.nrows != 0) { prod.push_back(Copy{dsc.src, dsc.nrows, dsc.copy_bytes}); continue; }
-        const SaChunk s = sa_prefix_chunk(hm.H, ncta, cta, dsc.sa_mode, L0, kv0, hm.n_tree, dsc.sa_item, dsc.sa_block);
-        if (s.nk == 0) continue;
-        prod.push_back(Copy{reinterpret_cast<const __half*>(dsc.src) + self_kv_index(s.j0, s.h * 64), 1u, s.nk * kv_bytes});
+      bool pf_ok = true;
+      uint64_t pending_bytes = 0;
+      ring_walk(
+          ctab.data(), need_a ? o[0] : o[1], prefill ? o[1] : o[3], o[1], o[3], l2_ahead, hm.H, hm.n_tree, cta, ncta, L0, kv0,
+          [&](const ChunkCopy& p) {
+            pending.push_back(p);
+            pending_bytes += (uint64_t)p.nrows * p.copy_bytes;
+            pf_ok = pf_ok && pending_bytes <= l2_ahead;
+          },
+          [&](const ChunkCopy& cp) {
+            prod.push_back(Copy{cp.src, cp.nrows, cp.copy_bytes});
+            // the copy must be of the oldest prefetched chunk, or (no budget) of one never prefetched
+            if (pf_head < pending.size() && same(pending[pf_head], cp)) {
+              pending_bytes -= (uint64_t)cp.nrows * cp.copy_bytes;
+              ++pf_head;
+            } else {
+              pf_ok = pf_ok && l2_ahead == 0;
+            }
+          });
+      // what is left was prefetched for the next launch: the tail program's leading weight chunks, in order
+      for (size_t i = pf_head, c = o[1]; i < pending.size() && pf_ok; ++i, ++c) {
+        pf_ok = (int)c < o[3] && ctab[c].nrows != 0 &&
+                same(pending[i], ChunkCopy{reinterpret_cast<const unsigned char*>(ctab[c].src), ctab[c].row_bytes,
+                                           ctab[c].nrows, ctab[c].copy_bytes});
       }
       for (int ip = need_a ? poff[0] : poff[1]; ip < (prefill ? poff[1] : poff[3]); ++ip) {
         const int stage = flat[ip * 3], mode = flat[ip * 3 + 1], layer = flat[ip * 3 + 2];
@@ -1840,7 +1870,7 @@ int dec_check_ring_schedule(const DecModel& hm, int ncta, int first[4]) {
             }
         }
       }
-      if (!(prod == cons)) {
+      if (!(prod == cons) || !pf_ok) {
         if (bad++ == 0) { first[0] = kv0; first[1] = L0; first[2] = need_a; first[3] = cta; }
       }
     }

@@ -159,6 +159,7 @@ struct RingGeom {
   static constexpr int ROW_STRIDE = D * 2 + 64;       // ring row stride, bytes
   // a slot holds 16 weight rows or the K (or V) rows of one cross-attention key chunk ([CH_PAD][72] fp16)
   static constexpr int SLOT_BYTES = (int)round128(cmax((size_t)16 * ROW_STRIDE, (size_t)WM_CH_PAD * 72 * sizeof(__half)));
+  static_assert(SLOT_BYTES <= WM_RING_SLOT_MAX && (D < 1280 || SLOT_BYTES == WM_RING_SLOT_MAX), "WM_RING_SLOT_MAX");
   static constexpr int XS = D * 4 + WM_XS_PADB;       // activation row stride, bytes
   static constexpr int NKS = ring_nks(D);             // k-slices per chunk (one MMA warp each)
   static constexpr int KS = D / NKS;
@@ -182,43 +183,115 @@ struct RingGeom {
 // ---------------------------------------------------------------------------------------------
 // producer warp: stream the chunk table through the ring
 // ---------------------------------------------------------------------------------------------
-// (L0, kv0: the loop state at launch, which sizes the self-attention prefix chunks)
-template <int D>
-__device__ __noinline__ void ring_producer(unsigned char* ring, uint64_t* full, uint64_t* empty,
-                                           const ChunkDesc* __restrict__ tab, int first, int last, const DecModel* m,
-                                           int cta, int ncta, int L0, int kv0) {
-  using G = RingGeom<D>;
-  const int lane = threadIdx.x & 31;
-  if (first >= last) return;
-  ChunkDesc nxt = tab[first];
-  int slot = 0;
-  unsigned int par = 1;   // parity to wait for on `empty` (fresh barrier: the "previous" phase counts as complete)
+// Bytes per CTA that the producer keeps prefetched into L2 ahead of its ring copies (ring_walk); chosen by A/B timing at
+// large-v2 (DESIGN.md section 4), and used on the whole GPU only (the clustered launch): on partial grids
+// (decode_ctas, StreamGroup) concurrent engines share HBM and L2, and the prefetch made four streams of 33 CTAs about
+// 10 % slower, so those launches run without it.  0 = no prefetch.  A nonzero budget holds at least the largest chunk, so the cursor
+// never stalls.  Full weight chunks at d = 1280 are 40,960 B, so 64 KB keeps about one chunk beyond the three slots in L2
+// (two when they are small): a fourth slot, in L2.
+#ifndef WM_RING_L2_AHEAD
+#define WM_RING_L2_AHEAD (64 * 1024)
+#endif
+static_assert(WM_RING_L2_AHEAD == 0 || WM_RING_L2_AHEAD >= WM_RING_SLOT_MAX, "the L2 lookahead must hold a whole chunk");
+
+// One ring chunk as a launch copies it: `nrows` rows of `copy_bytes`, row r read at src + r * row_bytes; nrows = 0:
+// nothing to copy (a self-attention prefix block that does not exist at this launch's (L0, kv0); the consumer skips it
+// too).  The producer's copies, its L2 prefetches and the host replay (dec_check_ring_schedule) all resolve chunks here.
+struct ChunkCopy { const unsigned char* src; uint32_t row_bytes, nrows, copy_bytes; };
+__host__ __device__ __forceinline__ ChunkCopy resolve_chunk(const ChunkDesc& dsc, int H, int n_tree, int cta, int ncta, int L0,
+                                                            int kv0) {
+  ChunkCopy c{reinterpret_cast<const unsigned char*>(dsc.src), dsc.row_bytes, dsc.nrows, dsc.copy_bytes};
+  if (dsc.nrows == 0) {
+    // a self-attention prefix block: one contiguous copy of its K or V rows
+    const SaChunk s = sa_prefix_chunk(H, ncta, cta, dsc.sa_mode, L0, kv0, n_tree, dsc.sa_item, dsc.sa_block);
+    c.nrows = s.nk > 0 ? 1u : 0u;
+    c.copy_bytes = (uint32_t)s.nk * WM_KV_ROW * sizeof(__half);
+    if (s.nk > 0) c.src += self_kv_index(s.j0, s.h * 64) * sizeof(__half);
+  }
+  return c;
+}
+
+// The producer's walk over chunks [first, last) of the chunk table (L0, kv0: the loop state at launch, which sizes the
+// self-attention prefix chunks).  copy(cp) puts a chunk into the next ring slot, waiting for the slot to free.  Before
+// each copy an L2 cursor tops up: it prefetches the chunks from the one about to be copied onwards while the bytes
+// prefetched but not yet copied stay within `budget`.  So HBM keeps streaming while the ring is full and the grid waits
+// at barriers, and a slot that frees is refilled from L2.  Past `last` the cursor goes on into the first weight chunks
+// of the tail program [warm_first, warm_last): the next launch starts there when this one's candidates are accepted,
+// and its first copies then hit L2 too.  It stops at the first self-attention prefix block there, which only the next
+// launch's loop state sizes.  A prefetch is a hint, and L2 is the point of coherence: no copy can read stale bytes.
+template <class Prefetch, class Copy>
+__host__ __device__ __forceinline__ void ring_walk(const ChunkDesc* tab, int first, int last, int warm_first, int warm_last,
+                                                   uint32_t budget, int H, int n_tree, int cta, int ncta, int L0, int kv0,
+                                                   Prefetch prefetch, Copy copy) {
+  int pf = first, pf_end = last;   // the cursor and the end of the range it walks
+  bool warm = false;               // walking the tail program
+  uint32_t ahead = 0;              // bytes prefetched, not yet copied
+  auto top_up = [&] {
+    while (budget > 0) {
+      if (pf == pf_end) {
+        if (warm) return;
+        warm = true; pf = warm_first; pf_end = warm_last;
+        continue;
+      }
+      const ChunkDesc& dsc = tab[pf];
+      if (warm && dsc.nrows == 0) { pf = pf_end; return; }
+      const ChunkCopy p = resolve_chunk(dsc, H, n_tree, cta, ncta, L0, kv0);
+      if (ahead + p.nrows * p.copy_bytes > budget) return;
+      if (p.nrows > 0) prefetch(p);
+      ahead += p.nrows * p.copy_bytes;
+      ++pf;
+    }
+  };
+  ChunkDesc nxt{};
+  if (first < last) nxt = tab[first];
   for (int c = first; c < last; ++c) {
     const ChunkDesc dsc = nxt;
-    if (c + 1 < last) nxt = tab[c + 1];                 // next descriptor is in flight while we wait
-    const unsigned char* src = reinterpret_cast<const unsigned char*>(dsc.src);
-    uint32_t nrows = dsc.nrows, copy_bytes = dsc.copy_bytes;
-    if (nrows == 0) {
-      // a self-attention prefix block: one contiguous copy of its K or V rows, or nothing (the consumer skips it too)
-      const SaChunk s = sa_prefix_chunk(m->H, ncta, cta, dsc.sa_mode, L0, kv0, m->n_tree, dsc.sa_item, dsc.sa_block);
-      if (s.nk == 0) continue;
-      src += self_kv_index(s.j0, s.h * 64) * sizeof(__half);
-      nrows = 1;
-      copy_bytes = (uint32_t)s.nk * WM_KV_ROW * sizeof(__half);
-    }
-    if (lane == 0) {
-      while (!mbar_try_wait(empty + slot, par)) { }
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic reads of the slot vs async writes
-      mbar_expect_tx(full + slot, nrows * copy_bytes);
-    }
-    __syncwarp();
-    if (lane < nrows) {
-      bulk_g2s(ring + (size_t)slot * G::SLOT_BYTES + (size_t)lane * G::ROW_STRIDE, src + (size_t)lane * dsc.row_bytes,
-               copy_bytes, full + slot);
-    }
-    __syncwarp();
-    if (++slot == WM_RING_G) { slot = 0; par ^= 1u; }
+    if (c + 1 < last) nxt = tab[c + 1];   // next descriptor is in flight while we wait
+    top_up();
+    const ChunkCopy cp = resolve_chunk(dsc, H, n_tree, cta, ncta, L0, kv0);
+    if (cp.nrows == 0) continue;
+    copy(cp);
+    if (budget > 0) ahead -= cp.nrows * cp.copy_bytes;
   }
+  top_up();
+}
+
+__device__ __forceinline__ void bulk_prefetch_l2(const void* src, uint32_t bytes) {
+  asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(src), "r"(bytes) : "memory");
+}
+
+template <int D>
+__device__ __noinline__ void ring_producer(unsigned char* ring, uint64_t* full, uint64_t* empty,
+                                           const ChunkDesc* __restrict__ tab, int first, int last, int warm_first,
+                                           int warm_last, const DecModel* m, int cta, int ncta, int L0, int kv0) {
+  using G = RingGeom<D>;
+  const int lane = threadIdx.x & 31;
+  int slot = 0;
+  unsigned int par = 1;   // parity to wait for on `empty` (fresh barrier: the "previous" phase counts as complete)
+  ring_walk(
+      tab, first, last, warm_first, warm_last, cluster_ncta() > 1 ? (uint32_t)WM_RING_L2_AHEAD : 0u, m->H, m->n_tree, cta, ncta, L0, kv0,
+      [&](const ChunkCopy& p) {
+        // one prefetch per contiguous range: the whole chunk, or each row of FC2's k-segment rows (as the copies go)
+        if (p.nrows == 1 || p.row_bytes == p.copy_bytes) {
+          if (lane == 0) bulk_prefetch_l2(p.src, p.nrows * p.copy_bytes);
+        } else if (lane < p.nrows) {
+          bulk_prefetch_l2(p.src + (size_t)lane * p.row_bytes, p.copy_bytes);
+        }
+      },
+      [&](const ChunkCopy& cp) {
+        if (lane == 0) {
+          while (!mbar_try_wait(empty + slot, par)) { }
+          asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic reads of the slot vs async writes
+          mbar_expect_tx(full + slot, cp.nrows * cp.copy_bytes);
+        }
+        __syncwarp();
+        if (lane < cp.nrows) {
+          bulk_g2s(ring + (size_t)slot * G::SLOT_BYTES + (size_t)lane * G::ROW_STRIDE, cp.src + (size_t)lane * cp.row_bytes,
+                   cp.copy_bytes, full + slot);
+        }
+        __syncwarp();
+        if (++slot == WM_RING_G) { slot = 0; par ^= 1u; }
+      });
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -760,8 +833,8 @@ dec_iteration_ring_kernel(const DecModel* __restrict__ gm) {
   if (warp == WM_DEC_THREADS / 32) {
     // ===== producer warp =====
     const int* off = m->chunk_off + cta * 4;
-    ring_producer<D>(smem, full, empty, m->chunk_tab, need_a ? off[0] : off[1], st->prefill ? off[1] : off[3], m, cta, ncta,
-                     L0, kv0);
+    ring_producer<D>(smem, full, empty, m->chunk_tab, need_a ? off[0] : off[1], st->prefill ? off[1] : off[3], off[1], off[3],
+                     m, cta, ncta, L0, kv0);
     return;
   }
 

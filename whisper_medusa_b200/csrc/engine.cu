@@ -1475,8 +1475,8 @@ extern "C" int wm_enc_gemm_tile(int32_t M, int32_t N, int32_t K, int32_t fp16_ou
   out3[0] = t[0]; out3[1] = t[1]; out3[2] = t[2];
   return WM_OK;
 }
-extern "C" int wm_ring_schedule_check(int32_t d_model, int32_t n_layers, int32_t medusa_block, int32_t K, int32_t n_tree,
-                                      int32_t n_cta, int32_t* n_bad, int32_t* first4) {
+static int ring_check(int32_t d_model, int32_t n_layers, int32_t medusa_block, int32_t K, int32_t n_tree, int32_t n_cta,
+                      long long l2_budget, int32_t* n_bad, int32_t* first4) {
   if (!n_bad || !first4 || d_model < 64 || d_model % 64 != 0 || n_layers < 1 || n_layers + 1 > WM_MAX_DEC_LAYERS || K < 1 ||
       n_tree < 1 || n_tree > WM_MAX_T || n_cta < 4 || n_cta > 1024)
     return WM_ERR_INVALID;
@@ -1497,7 +1497,17 @@ extern "C" int wm_ring_schedule_check(int32_t d_model, int32_t n_layers, int32_t
   fake(m.embed); fake(m.pos); fake(m.lnf_g); fake(m.lnf_b); fake(m.heads_w); fake(m.heads_b);
   fake(m.x); fake(m.xg); fake(m.q); fake(m.attn); fake(m.ffn_h); fake(m.hidden); fake(m.head_h); fake(m.carry);
   for (int i = 0; i < 4; ++i) first4[i] = -1;
-  *n_bad = dec_check_ring_schedule(m, n_cta, first4);
+  *n_bad = dec_check_ring_schedule(m, n_cta, l2_budget, first4);
   return WM_OK;
+}
+extern "C" int wm_ring_schedule_check(int32_t d_model, int32_t n_layers, int32_t medusa_block, int32_t K, int32_t n_tree,
+                                      int32_t n_cta, int32_t* n_bad, int32_t* first4) {
+  return ring_check(d_model, n_layers, medusa_block, K, n_tree, n_cta, -1, n_bad, first4);
+}
+extern "C" int wm_ring_prefetch_check(int32_t d_model, int32_t n_layers, int32_t medusa_block, int32_t K, int32_t n_tree,
+                                      int32_t n_cta, int32_t l2_budget, int32_t* n_bad, int32_t* first4) {
+  // a budget below one chunk would stall the cursor (the kernel's static_assert rules it out)
+  if (l2_budget < 0 || (l2_budget > 0 && l2_budget < WM_RING_SLOT_MAX)) return WM_ERR_INVALID;
+  return ring_check(d_model, n_layers, medusa_block, K, n_tree, n_cta, l2_budget, n_bad, first4);
 }
 extern "C" void* wm_weights_device_ptr(wm_handle* h) { return (h && h->wready) ? (void*)h->wdev : nullptr; }

@@ -38,7 +38,7 @@ struct ChunkDesc;
 void dec_build_ring_tables(const DecModel& hm, const float2* ln_fold, int ncta, int cluster, std::vector<CtaStage>& stab,
                            std::vector<ChunkDesc>& ctab, std::vector<int>& off);
 // host replay of the ring protocol over every launch state (wm_ring_schedule_check)
-int dec_check_ring_schedule(const DecModel& hm, int ncta, int first[4]);
+int dec_check_ring_schedule(const DecModel& hm, int ncta, long long l2_budget, int first[4]);   // l2_budget < 0: as built
 cudaError_t dec_launch_iteration_ring(const DecModel* dm, const DecHostInfo& hi, bool profile, cudaStream_t s);
 int dec_ring_cluster_size(const DecHostInfo& hi, int n_sm);
 // phase: 0 = sweep A over T uncached rows, 1 = tail (candidates), 2 = verify sweep + accept
