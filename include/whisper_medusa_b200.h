@@ -97,6 +97,20 @@ int wm_set_medusa_choices(wm_handle* h, const int32_t* choices, int32_t n);
 /* ---- logits processors (model.py:1168-1207; HF logits_process.py:1893-1901,1847-1862) -- */
 int wm_set_suppress(wm_handle* h, const int32_t* suppress_ids, int32_t n_suppress,
                     const int32_t* begin_suppress_ids, int32_t n_begin);
+/* HF's SequenceBias / NoBadWords / NoRepeatNGram / MinLength / MinNewTokens processors for the next wm_generate calls
+ * (until the next call of this function).  Sequence t is seq_tokens[seq_offsets[t] .. seq_offsets[t + 1]) with value
+ * seq_values[t]: a bias (finite), or -inf for a bad word; list sequence_bias's entries in dict order, then the bad
+ * words.  Every iteration adds to each row, before the EOS decay and the suppress masks, the values of the one-token
+ * sequences and of the longer ones whose prefix ends the iteration's starting sequence (fp32, in this order), and -inf
+ * for the tokens that followed the last no_repeat_ngram_size - 1 tokens anywhere in it, and for EOS while its length
+ * is below eos_min_length (max(min_length, prompt length + min_new_tokens)).  Every row of an iteration gets the same
+ * term, as in the reference.  Capacity: at most 256 sequences of two or more tokens, 4096 tokens among them
+ * (WM_ERR_UNSUPPORTED beyond); one-token sequences are not limited.  A token id >= vocab_size, a NaN or +inf value:
+ * WM_ERR_INVALID.  n_seqs = 0, no_repeat_ngram_size = 0 and eos_min_length <= 0: processors off (the default).
+ * wm_forward never applies them. */
+int wm_set_logits_processors(wm_handle* h, const int32_t* seq_tokens, const int32_t* seq_offsets,
+                             const float* seq_values, int32_t n_seqs, int32_t no_repeat_ngram_size,
+                             int32_t eos_min_length);
 
 /* ---- frontend + encoder (HF feature_extraction_whisper.py:135-164; modeling_whisper.py:593-647;
  *      cross-attention K/V projection :325-336) ------------------------------------------- */

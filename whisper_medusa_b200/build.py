@@ -20,7 +20,7 @@ LIB_PATH = os.path.join(OUT_DIR, "libwm_b200.so")
 ROOT = os.path.dirname(HERE)
 
 SOURCES = ["engine.cu", "decode.cu", "mel.cu", "enc_gemm.cu", "enc_attn.cu", "enc_gemm_tc.cu", "enc_attn_tc.cu",
-           "resample.cu", "scores.cu", "no_speech.cu", "timestamps.cu"]
+           "resample.cu", "scores.cu", "no_speech.cu", "timestamps.cu", "logits_proc.cu"]
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",

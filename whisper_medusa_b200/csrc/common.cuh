@@ -237,16 +237,34 @@ struct DecState {
   float row_pc[WM_MAX_T];        // [n]: softmax prob of node n's token in the posterior of its parent row (chain: parent = n-1)
   float row_thr[WM_MAX_T];
   int path_node;    // tree mode: node path[accept] of the best candidate of the last iteration (read by the scoring kernel)
+  // logits processors (wm_set_logits_processors): the address of the iteration's adj[V] (dec_state_adj), written by
+  // logits_proc.cu before each iteration; 0 = off for the whole call (the logits scans then run their variant without
+  // it).  Kept here rather than in DecModel, whose size the ring kernel's shared-memory copy depends on, and as two
+  // 32-bit words so that DecState keeps its 4-byte alignment (with an 8-byte member the loop kernels compile to
+  // different register allocations).
+  unsigned int adj_lo, adj_hi;
 };
+__host__ __device__ __forceinline__ const float* dec_state_adj(const DecState* st) {
+  return reinterpret_cast<const float*>(((unsigned long long)st->adj_hi << 32) | st->adj_lo);
+}
+__host__ __device__ __forceinline__ void dec_state_set_adj(DecState* st, const float* adj) {
+  const unsigned long long a = reinterpret_cast<unsigned long long>(adj);
+  st->adj_lo = (unsigned int)a;
+  st->adj_hi = (unsigned int)(a >> 32);
+}
 
 // Logits processors applied to element j of a raw logits row, with cur_len = L (HF logits_process.py:1893-1901 suppress,
 // :1847-1862 begin-suppress when L == begin_index, :1742-1772 EOS exponential decay with pen = pen_tab[L]).  Shared by
-// the loop's logits scan and the scoring kernel.
+// the loop's logits scan and the scoring kernel.  ADJ: the iteration's per-token term adj[V] of the sequence-bias,
+// bad-words, no-repeat-n-gram and min-length processors (logits_proc.cu) is added first, as HF's chain adds it before
+// the decay.  Callers instantiate both variants and pick one with a uniform flag, so the off path is today's code.
+template <bool ADJ = false>
 __device__ __forceinline__ float processed_logit(const float* row, int j, const uint8_t* mask, bool begin_on,
-                                                 int eos, float pen) {
+                                                 int eos, float pen, const float* adj = nullptr) {
   const uint8_t mk = mask[j];
   if ((mk & 1) || (begin_on && (mk & 2))) return -INFINITY;
   float v = ldcg_f(row + j);
+  if (ADJ) v = v + ldcg_f(adj + j);
   if (j == eos && pen != 0.f) v = v + fabsf(v) * pen;
   return v;
 }

@@ -947,7 +947,8 @@ __device__ __forceinline__ int select_nseg(const DecModel* m, int /*ncta*/) { re
 // strict "comes after" in the candidate order (value descending, index ascending)
 __device__ __forceinline__ bool ranks_after(float v, int i, float pv, int pi) { return v < pv || (v == pv && i > pi); }
 
-__device__ __noinline__ void stage_select1(const DecModel* m, int mode, int cta, int ncta, unsigned char* smem_raw) {
+template <bool ADJ>
+__device__ __noinline__ void stage_select1_rows(const DecModel* m, int mode, int cta, int ncta, unsigned char* smem_raw) {
   const DecState* st = m->st;
   const int V = m->V, K = m->K;
   float* s_val = reinterpret_cast<float*>(smem_raw);
@@ -956,6 +957,7 @@ __device__ __noinline__ void stage_select1(const DecModel* m, int mode, int cta,
   const bool begin_on = (L == st->begin_index);
   const float pen = m->pen_tab[L];
   const int eos = st->eos;
+  const float* adj = ADJ ? dec_state_adj(st) : nullptr;
   const float* logits = (mode == MODE_A) ? m->logits_a : m->logits_b;
   const int nseg = select_nseg(m, ncta);
   const int seglen = (V + nseg - 1) / nseg;
@@ -971,14 +973,14 @@ __device__ __noinline__ void stage_select1(const DecModel* m, int mode, int cta,
     float bv = -INFINITY;
     int bi = 0x7fffffff;
     for (int j = j0 + threadIdx.x; j < j1; j += WM_DEC_THREADS) {
-      const float v = processed_logit(row, j, m->tok_mask, begin_on, eos, pen);
+      const float v = processed_logit<ADJ>(row, j, m->tok_mask, begin_on, eos, pen, adj);
       if (v > bv) { bv = v; bi = j; }   // ascending j per thread => first maximum kept
     }
     block_argmax(bv, bi, s_val, s_idx);
     float z = 0.f;
     if (mode == MODE_B && r < n_stat && temp > 0.f && bv > -INFINITY) {
       for (int j = j0 + threadIdx.x; j < j1; j += WM_DEC_THREADS)
-        z += expf((processed_logit(row, j, m->tok_mask, begin_on, eos, pen) - bv) * inv_t);
+        z += expf((processed_logit<ADJ>(row, j, m->tok_mask, begin_on, eos, pen, adj) - bv) * inv_t);
       z = block_sum(z, s_val);
     }
     if (threadIdx.x == 0) {
@@ -995,7 +997,7 @@ __device__ __noinline__ void stage_select1(const DecModel* m, int mode, int cta,
       for (int q = 1; q < kk; ++q) {
         float cv = -INFINITY; int ci = 0x7fffffff;
         for (int j = j0 + threadIdx.x; j < j1; j += WM_DEC_THREADS) {
-          const float v = processed_logit(row, j, m->tok_mask, begin_on, eos, pen);
+          const float v = processed_logit<ADJ>(row, j, m->tok_mask, begin_on, eos, pen, adj);
           if (ranks_after(v, j, pv, pi) && (v > cv)) { cv = v; ci = j; }
         }
         block_argmax(cv, ci, s_val, s_idx);
@@ -1031,7 +1033,8 @@ __device__ __forceinline__ void select_fold(const DecModel* m, int r, int nseg, 
   }
 }
 
-__device__ __noinline__ void stage_select2(const DecModel* m, int cta, int ncta, unsigned char* smem_raw) {
+template <bool ADJ>
+__device__ __noinline__ void stage_select2_rows(const DecModel* m, int cta, int ncta, unsigned char* smem_raw) {
   DecState* st = m->st;
   const int V = m->V, K = m->K;
   float* s_val = reinterpret_cast<float*>(smem_raw);
@@ -1042,6 +1045,7 @@ __device__ __noinline__ void stage_select2(const DecModel* m, int cta, int ncta,
   const bool begin_on = (L == st->begin_index);
   const float pen = m->pen_tab[L];
   const int eos = st->eos;
+  const float* adj = ADJ ? dec_state_adj(st) : nullptr;
   const int nseg = select_nseg(m, ncta);
   const int seglen = (V + nseg - 1) / nseg;
   const bool tree = m->has_tree != 0;
@@ -1054,7 +1058,7 @@ __device__ __noinline__ void stage_select2(const DecModel* m, int cta, int ncta,
     select_fold(m, r, nseg, inv_t, M, idx, Z, ent_unused);   // (every warp folds the same row: uniform)
     float ent = 0.f;
     for (int j = j0 + threadIdx.x; j < j1; j += WM_DEC_THREADS) {
-      const float p = expf((processed_logit(row, j, m->tok_mask, begin_on, eos, pen) - M) * inv_t) / Z;
+      const float p = expf((processed_logit<ADJ>(row, j, m->tok_mask, begin_on, eos, pen, adj) - M) * inv_t) / Z;
       ent += p * logf(p + 1e-5f);
     }
     ent = block_sum(ent, s_val);
@@ -1066,10 +1070,22 @@ __device__ __noinline__ void stage_select2(const DecModel* m, int cta, int ncta,
         if (tree && m->tree->parent[n] != r) continue;
         const int c = ldcg_i(&st->cand[n]);
         if (c >= j0 && c < j1)
-          st->row_pc[n] = expf((processed_logit(row, c, m->tok_mask, begin_on, eos, pen) - M) * inv_t) / Z;
+          st->row_pc[n] = expf((processed_logit<ADJ>(row, c, m->tok_mask, begin_on, eos, pen, adj) - M) * inv_t) / Z;
       }
     }
   }
+}
+
+// The variant with the logits-processor term, or without it, chosen by the uniform DecState adj (on / off for the whole
+// call): the stage and persistent kernels.  The ring kernel is instantiated with and without processors instead, so its
+// variant without them is the same code as a build without processors.
+__device__ __noinline__ void stage_select1(const DecModel* m, int mode, int cta, int ncta, unsigned char* smem_raw) {
+  if (dec_state_adj(m->st)) stage_select1_rows<true>(m, mode, cta, ncta, smem_raw);
+  else stage_select1_rows<false>(m, mode, cta, ncta, smem_raw);
+}
+__device__ __noinline__ void stage_select2(const DecModel* m, int cta, int ncta, unsigned char* smem_raw) {
+  if (dec_state_adj(m->st)) stage_select2_rows<true>(m, cta, ncta, smem_raw);
+  else stage_select2_rows<false>(m, cta, ncta, smem_raw);
 }
 
 // tail: candidates = top-1 of every head row (generate_candidates, medusa_utils.py:446-457)
@@ -1415,8 +1431,9 @@ __host__ __device__ GemmDesc make_gemm_desc(const DecModel* m, int stage, int mo
 }
 
 // WITH_GEMM = false: the caller runs the GEMM stages itself (ring kernel) -- keeps stage_gemm out of
-// that kernel's code
-template <bool WITH_GEMM = true>
+// that kernel's code.  ADJ: the logits scans with (1) or without (0) the logits-processor term, or chosen at run time
+// from dec_state_adj (-1)
+template <bool WITH_GEMM = true, int ADJ = -1>
 __device__ void run_stage(const DecModel* m, int stage, int mode, int layer, int cta, int ncta, unsigned char* smem,
                           const PassGeom* gopt = nullptr, unsigned long long* pr = nullptr) {
   switch (stage) {
@@ -1426,8 +1443,14 @@ __device__ void run_stage(const DecModel* m, int stage, int mode, int layer, int
     case ST_FINAL_LN: stage_final_ln(m, mode, cta, ncta, gopt); break;
     case ST_COPY_HIDDEN: stage_copy_hidden_to_x(m, mode, cta, ncta, gopt); break;
     case ST_TAIL_SEED: stage_tail_seed(m, cta, ncta); break;
-    case ST_SELECT1: stage_select1(m, mode, cta, ncta, smem); break;
-    case ST_SELECT2: stage_select2(m, cta, ncta, smem); break;
+    case ST_SELECT1:
+      if (ADJ < 0) stage_select1(m, mode, cta, ncta, smem);
+      else stage_select1_rows<(ADJ > 0)>(m, mode, cta, ncta, smem);
+      break;
+    case ST_SELECT2:
+      if (ADJ < 0) stage_select2(m, cta, ncta, smem);
+      else stage_select2_rows<(ADJ > 0)>(m, cta, ncta, smem);
+      break;
     case ST_SELECT_FIN: if (cta == 0) stage_select_fin(m, ncta); break;
     case ST_ACCEPT:
       if (cta == 0) { if (m->has_tree) stage_accept_tree(m, ncta); else stage_accept(m, ncta); }
@@ -1891,9 +1914,13 @@ cudaError_t dec_relayout_cross_kv(const __half* kv, __half* ck, __half* cv, int 
   return cudaGetLastError();
 }
 
-static void* ring_kernel_fn(int d, bool profile) {
+// profile: the stage-timeline variant (processors chosen at run time); lp: the variant with logits processors
+static void* ring_kernel_fn(int d, bool profile, bool lp = false) {
   switch (d) {
-#define WM_CASE(DD) case DD: return profile ? (void*)dec_iteration_ring_kernel<DD, true> : (void*)dec_iteration_ring_kernel<DD, false>;
+#define WM_CASE(DD)                                                                                                          \
+  case DD:                                                                                                                   \
+    return profile ? (void*)dec_iteration_ring_kernel<DD, true, false>                                                      \
+                   : lp ? (void*)dec_iteration_ring_kernel<DD, false, true> : (void*)dec_iteration_ring_kernel<DD, false, false>;
     WM_RING_WIDTHS(WM_CASE)
 #undef WM_CASE
     default: return nullptr;
@@ -1902,7 +1929,7 @@ static void* ring_kernel_fn(int d, bool profile) {
 
 // Cooperative launch (the grid barrier needs every CTA resident), as clusters of hi.cluster CTAs along x.
 cudaError_t dec_launch_iteration_ring(const DecModel* dm, const DecHostInfo& hi, bool profile, cudaStream_t s) {
-  void* fn = ring_kernel_fn(hi.d, profile);
+  void* fn = ring_kernel_fn(hi.d, profile, hi.lp != 0);
   if (!fn) return cudaErrorInvalidValue;
   void* args[] = {(void*)&dm};
   cudaLaunchAttribute attr[2];
@@ -1964,9 +1991,11 @@ cudaError_t dec_configure(int d, size_t smem, size_t smem_ring) {
   switch (d) {
 #define WM_CASE(DD)                                                                                                          \
   case DD:                                                                                                                   \
-    e = cudaFuncSetAttribute(dec_iteration_ring_kernel<DD, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_ring); \
+    e = cudaFuncSetAttribute(dec_iteration_ring_kernel<DD, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_ring); \
     if (e != cudaSuccess) return e;                                                                                          \
-    return cudaFuncSetAttribute(dec_iteration_ring_kernel<DD, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_ring);
+    e = cudaFuncSetAttribute(dec_iteration_ring_kernel<DD, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_ring); \
+    if (e != cudaSuccess) return e;                                                                                          \
+    return cudaFuncSetAttribute(dec_iteration_ring_kernel<DD, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_ring);
     WM_RING_WIDTHS(WM_CASE)
 #undef WM_CASE
     default: return cudaErrorInvalidValue;

@@ -127,6 +127,9 @@ struct wm_handle {
   int* ts_jumps = nullptr;      // [WM_TS_MAX_N]
   float* ts_times = nullptr;    // [WM_TS_MAX_N + 1]
   int last_ts = 0, last_ts_tree = 0;   // 1: the last wm_generate captured the listed pairs (on a branching tree)
+  // logits processors (wm_set_logits_processors); buffers allocated on first use
+  int lp_on = 0;
+  LogitsProcArgs lp{};          // device tables: base [V], adj [V], seq_tok / seq_off / seq_val (WM_LP_MAX_* entries)
 };
 
 #define WM_TS_MAX_LIST 64   // alignment pairs per call (duplicates included)
@@ -412,6 +415,7 @@ extern "C" int wm_destroy(wm_handle* h) {
   F(h->hm.topk_part); F(h->tree); F(h->hm.logits_a); F(h->hm.logits_b); F(h->st); F(h->tok_mask); F(h->pen_tab); F(h->bar); F(h->prof); F(h->chunk_tab); F(h->chunk_off); F(h->stage_tab); F(h->ln_fold); F(h->dm);
   F(h->score_state); F(h->score_part); F(h->score_lp); F(h->score_rows);
   F(h->hm.ns_hidden); F(h->ns_head); F(h->ns_logits); F(h->ns_part); F(h->ns_count);
+  F(h->lp.base); F(h->lp.adj); F(h->lp.seq_tok); F(h->lp.seq_off); F(h->lp.seq_val);
   F(h->ts_dev); F(h->ts_scores); F(h->ts_head_slot); F(h->ts_probs); F(h->ts_matrix); F(h->ts_jumps); F(h->ts_times);
   if (h->wowned) F(h->wdev);
   for (auto& kv : h->resamplers) { F(kv.second.taps); F(kv.second.sup); }
@@ -930,6 +934,7 @@ extern "C" int wm_generate(wm_handle* h, const int32_t* prompt, int32_t n_prompt
     hs.begin_index = gp->begin_index; hs.temperature = gp->temperature; hs.post_thr = gp->posterior_threshold;
     hs.post_alpha = gp->posterior_alpha;
     hs.tree_attn = (h->hm.has_tree && gp->tree_attention) ? 1 : 0;
+    dec_state_set_adj(&hs, h->lp_on ? h->lp.adj : nullptr);
     for (int i = 0; i < n_prompt; ++i) hs.ids[i] = prompt[i];
     // reference stop rule evaluated before the first iteration is never true for sane inputs; the
     // loop always runs at least once (model.py:635).
@@ -943,11 +948,16 @@ extern "C" int wm_generate(wm_handle* h, const int32_t* prompt, int32_t n_prompt
   ScoreArgs sa;
   memset(&sa, 0, sizeof sa);
   sa.logits_a = h->hm.logits_a; sa.logits_b = h->hm.logits_b; sa.st = h->st; sa.tree = h->hm.has_tree ? h->tree : nullptr;
-  sa.tok_mask = h->tok_mask; sa.pen_tab = h->pen_tab; sa.V = h->cfg.vocab_size; sa.n_prompt = n_prompt;
+  sa.tok_mask = h->tok_mask; sa.pen_tab = h->pen_tab; sa.adj = dec_state_adj(h->h_init); sa.V = h->cfg.vocab_size; sa.n_prompt = n_prompt;
   sa.want_lp = score_bits & 1; sa.want_rows = (score_bits >> 1) & 1;
   sa.state = h->score_state; sa.part = h->score_part; sa.lp = h->score_lp; sa.rows = h->score_rows;
   sa.cap_rows = h->cfg.max_target_positions;
   const int score_grid = dec_score_grid(h->n_cta, K);
+  const bool lp_on = dec_state_adj(h->h_init) != nullptr;
+  h->hi.lp = lp_on;   // (prefill launches only run sweep A: no logits scan)
+  LogitsProcArgs la = h->lp;
+  la.st = h->st;
+  const int lp_grid = dec_logits_proc_grid(h->n_cta);
   // Long prompts (decoder_input_ids beyond the 16 rows of a stage tile): the leading tokens are cached by prefill
   // launches -- sweep A over 16-token chunks, no candidates / verify -- before the loop proper starts on the rest.
   int n_tail = n_prompt;     // rows of the first real iteration's sweep A
@@ -993,6 +1003,10 @@ extern "C" int wm_generate(wm_handle* h, const int32_t* prompt, int32_t n_prompt
     if (gp->max_iters > 0 && lb > gp->max_iters - iters) lb = gp->max_iters - iters;
     if (lb < 1) lb = 1;
     for (int i = 0; i < lb; ++i) {
+      if (lp_on) {   // this iteration's adj from the sequence it starts with; a no-op once the loop has ended
+        CK(dec_launch_logits_proc(la, lp_grid, s));
+        h->launches[2] += 1;
+      }
       const int64_t nl = enqueue_iteration(h, h->decode_mode, iters + i == 0 ? n_tail : 1, 2, h->hm.prof != nullptr);
       if (nl < 0) return (int)nl;
       h->launches[2] += nl;
@@ -1091,6 +1105,61 @@ extern "C" int wm_set_alignment_heads(wm_handle* h, const int32_t* pairs, int32_
   for (int i = 0; i < h->cfg.dec_layers * H; ++i) tc[0].slot[i] = slot_of[i];
   CK(cudaMemcpy(h->ts_dev, tc.data(), sizeof(TsCapture), cudaMemcpyHostToDevice));
   CK(cudaMemcpy(h->ts_head_slot, list_slot.data(), (size_t)n_pairs * sizeof(int), cudaMemcpyHostToDevice));
+  return WM_OK;
+}
+
+extern "C" int wm_set_logits_processors(wm_handle* h, const int32_t* seq_tokens, const int32_t* seq_offsets,
+                                        const float* seq_values, int32_t n_seqs, int32_t no_repeat_ngram_size,
+                                        int32_t eos_min_length) {
+  if (!h || n_seqs < 0 || no_repeat_ngram_size < 0) return WM_ERR_INVALID;
+  if (n_seqs > 0 && (!seq_tokens || !seq_offsets || !seq_values)) return WM_ERR_INVALID;
+  const int V = h->cfg.vocab_size;
+  std::vector<float> base;
+  std::vector<int> tok, off(1, 0);
+  std::vector<float> val;
+  if (n_seqs > 0) {
+    if (seq_offsets[0] != 0) return fail(h, WM_ERR_INVALID, "seq_offsets[0] must be 0");
+    base.assign(V, 0.f);
+    for (int t = 0; t < n_seqs; ++t) {
+      const int o = seq_offsets[t], len = seq_offsets[t + 1] - o;
+      if (len < 1) return fail(h, WM_ERR_INVALID, "every logits-processor sequence needs at least one token");
+      for (int k = 0; k < len; ++k)
+        if (seq_tokens[o + k] < 0 || seq_tokens[o + k] >= V) return fail(h, WM_ERR_INVALID, "sequence token id out of range");
+      const float v = seq_values[t];
+      if (std::isnan(v) || v == INFINITY) return fail(h, WM_ERR_INVALID, "sequence values must be finite or -inf");
+      if (len == 1) { base[seq_tokens[o]] += v; continue; }   // (sums in table order, from zero, as HF's bias)
+      if ((int)val.size() == WM_LP_MAX_SEQS || (int)tok.size() + len > WM_LP_MAX_TOKENS)
+        return fail(h, WM_ERR_UNSUPPORTED, "more than 256 multi-token sequences or 4096 of their tokens");
+      tok.insert(tok.end(), seq_tokens + o, seq_tokens + o + len);
+      off.push_back((int)tok.size());
+      val.push_back(v);
+    }
+  }
+  const bool on = n_seqs > 0 || no_repeat_ngram_size > 0 || eos_min_length > 0;
+  if (!on && !h->lp_on) return WM_OK;
+  if (h->device < 0) return fail(h, WM_ERR_STATE, "layout-only handle");
+  CK(cudaSetDevice(h->device));
+  CK(cudaStreamSynchronize(h->stream));   // (no loop may read the tables while they are rewritten)
+  h->lp_on = on;
+  if (!on) return WM_OK;                  // wm_generate switches the processors off
+  if (!h->lp.adj) {
+    CK(dalloc(&h->lp.base, (size_t)V));
+    CK(dalloc(&h->lp.adj, (size_t)V));
+    CK(dalloc(&h->lp.seq_tok, WM_LP_MAX_TOKENS));
+    CK(dalloc(&h->lp.seq_off, WM_LP_MAX_SEQS + 1));
+    CK(dalloc(&h->lp.seq_val, WM_LP_MAX_SEQS));
+  }
+  if (base.empty()) CK(cudaMemset(h->lp.base, 0, (size_t)V * sizeof(float)));
+  else CK(cudaMemcpy(h->lp.base, base.data(), (size_t)V * sizeof(float), cudaMemcpyHostToDevice));
+  if (!val.empty()) {
+    CK(cudaMemcpy(h->lp.seq_tok, tok.data(), tok.size() * sizeof(int), cudaMemcpyHostToDevice));
+    CK(cudaMemcpy(h->lp.seq_off, off.data(), off.size() * sizeof(int), cudaMemcpyHostToDevice));
+    CK(cudaMemcpy(h->lp.seq_val, val.data(), val.size() * sizeof(float), cudaMemcpyHostToDevice));
+  }
+  h->lp.n_seq = (int)val.size();
+  h->lp.ngram = no_repeat_ngram_size;
+  h->lp.eos_min_len = eos_min_length;
+  h->lp.V = V;
   return WM_OK;
 }
 
@@ -1272,6 +1341,7 @@ extern "C" int wm_forward(wm_handle* h, const int32_t* ids, int32_t n_ids, float
   const int K = h->cfg.medusa_num_heads;
   const size_t V = (size_t)h->cfg.vocab_size;
   h->st_from_generate = 0;   // the loop state is rewritten below
+  h->hi.lp = 0;              // (no logits processors: the state below has no adj)
   {
     const int r = set_ts_capture(h, false);   // (the passes below must not overwrite the last wm_generate's captured
     if (r != WM_OK) return r;                  //  alignment rows, nor its no-speech row)

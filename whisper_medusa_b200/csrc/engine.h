@@ -18,6 +18,7 @@ struct DecHostInfo {
   size_t smem;
   size_t smem_ring;
   int cluster = 1; // CTAs per cluster of the ring kernel (1 or 2, dec_ring_cluster_size)
+  int lp = 0;      // 1: logits processors on for the iterations enqueued next (the ring kernel's variant with them)
 };
 
 // ---- decode.cu ----
@@ -59,6 +60,7 @@ struct ScoreArgs {
   const DecTree* tree;     // null for a chain
   const uint8_t* tok_mask;
   const float* pen_tab;
+  const float* adj;        // logits-processor term of the iteration (dec_state_adj), null = processors off
   int V;
   int n_prompt;            // first position scored (prefill launches of a long prompt are not scored)
   int want_lp, want_rows;  // option "scores" bit 0 / bit 1
@@ -70,6 +72,28 @@ struct ScoreArgs {
 };
 int dec_score_grid(int n_cta, int K);
 cudaError_t dec_launch_scores(const ScoreArgs& a, int grid, cudaStream_t s);
+
+// ---- logits_proc.cu ----
+#define WM_LP_THREADS 256
+#define WM_LP_MAX_SEQS 256       // multi-token sequences of sequence_bias + bad_words_ids (wm_set_logits_processors)
+#define WM_LP_MAX_TOKENS 4096    // their tokens in all
+// What the logits-processor kernel reads and writes; one launch before each speculative iteration while processors are
+// on.  adj[j] = base[j] + the values of the multi-token sequences whose prefix ends the sequence (in table order), or
+// -inf for a no-repeat-n-gram ban or the EOS ban of min_length / min_new_tokens.
+struct LogitsProcArgs {
+  const DecState* st;
+  float* base;             // [V] single-token biases (sums in table order; -inf for a banned token)
+  int* seq_tok;            // multi-token sequences, flattened
+  int* seq_off;            // [n_seq + 1]
+  float* seq_val;          // [n_seq] bias, or -inf for a bad word
+  int n_seq;
+  int ngram;               // no_repeat_ngram_size, 0 = off
+  int eos_min_len;         // EOS is banned while len(input_ids) < eos_min_len
+  int V;
+  float* adj;              // [V]
+};
+int dec_logits_proc_grid(int n_cta);
+cudaError_t dec_launch_logits_proc(const LogitsProcArgs& a, int grid, cudaStream_t s);
 
 // ---- no_speech.cu ----
 #define WM_NS_NSEG 512         // vocabulary segments of the no-speech row (fixed: the fold order does not depend on the grid)

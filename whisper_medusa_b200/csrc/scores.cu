@@ -4,7 +4,8 @@
 // logits_a (the tail's rows), logits_b (the verify rows) and the loop state -- and keeps its own cursor (the first
 // position not scored yet), so an iteration that did not run (the loop ended earlier in the batch) costs one early
 // return.  With L0 = the cursor (len(input_ids) at the start of the iteration), a = the accept length and path = the
-// best candidate's root-to-leaf nodes, every row is processed with cur_len = L0 (processed_logit) and:
+// best candidate's root-to-leaf nodes, every row is processed with cur_len = L0 (processed_logit, with the iteration's
+// logits-processor term adj when processors are on) and:
 //   token at L0          (c0)                 <- base row 0 of the tail (logits_a)
 //   token at L0 + j, j>=1 (c1..ca / the extra) <- verify row path[j - 1]
 //   scores row of the iteration              <- verify row path[a] (the reference's next_token_logits)
@@ -35,6 +36,7 @@ __device__ __forceinline__ int path_node(const DecState* st, const DecTree* tree
   return node;
 }
 
+template <bool ADJ>
 __global__ void __launch_bounds__(WM_SCORE_THREADS) score_iteration_kernel(ScoreArgs p) {
   constexpr int NW = WM_SCORE_THREADS / 32;
   __shared__ float s_m[NW], s_s[NW];
@@ -61,13 +63,13 @@ __global__ void __launch_bounds__(WM_SCORE_THREADS) score_iteration_kernel(Score
     if (r == n_lp) {   // the scores row: the processed verify row path[a]
       const float* row = p.logits_b + (size_t)path_node(st, p.tree, a, a) * V;
       float* out = p.rows + (size_t)(it - 1) * V;
-      for (int j = j0 + threadIdx.x; j < j1; j += WM_SCORE_THREADS) out[j] = processed_logit(row, j, p.tok_mask, begin_on, eos, pen);
+      for (int j = j0 + threadIdx.x; j < j1; j += WM_SCORE_THREADS) out[j] = processed_logit<ADJ>(row, j, p.tok_mask, begin_on, eos, pen, p.adj);
       continue;
     }
     const float* row = (r == 0) ? p.logits_a : p.logits_b + (size_t)path_node(st, p.tree, a, r - 1) * V;
     if (threadIdx.x == 0) {   // the segment holding the row's token also records its processed logit for the fold
       const int tok = st->ids[L0 + r];
-      if (tok >= j0 && tok < j1) p.part[(size_t)(WM_MAX_T + 1) * WM_SCORE_NSEG * 2 + r] = processed_logit(row, tok, p.tok_mask, begin_on, eos, pen);
+      if (tok >= j0 && tok < j1) p.part[(size_t)(WM_MAX_T + 1) * WM_SCORE_NSEG * 2 + r] = processed_logit<ADJ>(row, tok, p.tok_mask, begin_on, eos, pen, p.adj);
     }
     float m = -INFINITY, s = 0.f;
     // WM_SCORE_UNROLL elements per thread in flight at once: the segment is read from L2, and one element at a time
@@ -77,7 +79,7 @@ __global__ void __launch_bounds__(WM_SCORE_THREADS) score_iteration_kernel(Score
 #pragma unroll
       for (int u = 0; u < WM_SCORE_UNROLL; ++u) {
         const int j = jb + u * WM_SCORE_THREADS;
-        v[u] = j < j1 ? processed_logit(row, j, p.tok_mask, begin_on, eos, pen) : -INFINITY;
+        v[u] = j < j1 ? processed_logit<ADJ>(row, j, p.tok_mask, begin_on, eos, pen, p.adj) : -INFINITY;
       }
 #pragma unroll
       for (int u = 0; u < WM_SCORE_UNROLL; ++u) {
@@ -134,7 +136,8 @@ __global__ void __launch_bounds__(WM_SCORE_THREADS) score_iteration_kernel(Score
 int dec_score_grid(int n_cta, int K) { return std::min(n_cta, (K + 2) * WM_SCORE_NSEG); }
 
 cudaError_t dec_launch_scores(const ScoreArgs& a, int grid, cudaStream_t s) {
-  score_iteration_kernel<<<grid, WM_SCORE_THREADS, 0, s>>>(a);
+  if (a.adj) score_iteration_kernel<true><<<grid, WM_SCORE_THREADS, 0, s>>>(a);
+  else score_iteration_kernel<false><<<grid, WM_SCORE_THREADS, 0, s>>>(a);
   return cudaGetLastError();
 }
 

@@ -34,6 +34,7 @@ from . import _lib
 from .config import MedusaConfig, MedusaGenerationConfig
 from .longform import (MAX_WINDOW_SAMPLES, SAMPLE_RATE, Window, WindowResult, merge_timed, merge_windows,
                        no_speech_rule, plan_windows, resampled_length, skip_window, window_params)
+from . import processors as _processors
 from .weights import pack_blob
 
 N_FRAMES = 3000
@@ -479,6 +480,7 @@ class WhisperMedusaModel:
         if input_features.shape[-1] != N_FRAMES or input_features.shape[-2] != self.config.num_mel_bins:
             raise ValueError(f"input_features must be [1, {self.config.num_mel_bins}, {N_FRAMES}] (WhisperProcessor output)")
         self._check_unsupported(temperature, attention_mask, kwargs)
+        self._logits_processors(kwargs, generation_config)
         num_frames = self._mask_frames(attention_mask) if attention_mask is not None else None
         ts = self._timestamp_request(generation_config, task, num_frames, time_precision) if return_token_timestamps else None
         self._encode_features(input_features)
@@ -555,10 +557,50 @@ class WhisperMedusaModel:
             raise NotImplementedError("sampling (temperature > 0 / do_sample) is not supported with medusa: greedy search only")
         known = {"exponential_decay_length_penalty", "max_length", "max_new_tokens", "max_iters", "medusa_temperature",
                  "posterior_threshold", "posterior_alpha", "num_beams", "do_sample", "use_cache", "tree_attention",
-                 "decoder_input_ids", "output_scores", "output_logits", "output_no_speech_prob"}
+                 "decoder_input_ids", "output_scores", "output_logits", "output_no_speech_prob", *_processors.KEYS}
         unknown = sorted(set(kwargs) - known)
         if unknown:
             raise NotImplementedError(f"generate() options not implemented by the H100 engine: {unknown}")
+
+    def _logits_processors(self, kwargs, generation_config=None,
+                           prompt: Optional[Sequence[int]] = None) -> Optional[_processors.Processors]:
+        """The call's ``sequence_bias`` / ``bad_words_ids`` / ``no_repeat_ngram_size`` / ``min_length`` /
+        ``min_new_tokens`` (kwargs, else the generation config's attributes), checked, as engine tables; None = off.
+        Without ``prompt`` (checks before any GPU work) the prompt length is the one ``_decode`` will use."""
+        g = generation_config if generation_config is not None else self.generation_config
+        if prompt is not None:
+            n_prompt = len(prompt)
+        elif kwargs.get("decoder_input_ids") is not None:
+            n_prompt = int(torch.as_tensor(kwargs["decoder_input_ids"]).numel())
+        else:
+            n_prompt = 4 if g.is_multilingual else 2      # _init_tokens
+        max_length = kwargs.get("max_length") if kwargs.get("max_length") is not None else g.max_length
+        if kwargs.get("max_new_tokens") is not None:
+            max_length = n_prompt + int(kwargs["max_new_tokens"])
+        pen = kwargs.get("exponential_decay_length_penalty")
+        pen = pen if pen is not None else g.exponential_decay_length_penalty
+        return _processors.build(_processors.options(kwargs, g), int(g.eos_token_id), int(self.config.vocab_size),
+                                 n_prompt, int(max_length), pen)
+
+    def _push_logits_processors(self, procs: Optional[_processors.Processors]) -> None:
+        """Sent on every call that has processors, and switched off again on the engine that last had them, so a call
+        without processors launches nothing extra."""
+        if procs is None and getattr(self, "_lp_engine", None) != self._handle.value:
+            return
+        lib = _lib.load()
+        seqs = procs.seqs if procs is not None else []
+        toks = [t for ids, _ in seqs for t in ids]
+        offs = [0]
+        for ids, _ in seqs:
+            offs.append(offs[-1] + len(ids))
+        _check(lib, self._handle,
+               lib.wm_set_logits_processors(self._handle, (C.c_int32 * max(1, len(toks)))(*toks),
+                                            (C.c_int32 * len(offs))(*offs),
+                                            (C.c_float * max(1, len(seqs)))(*[v for _, v in seqs]), len(seqs),
+                                            procs.ngram if procs is not None else 0,
+                                            procs.eos_min_length if procs is not None else 0),
+               "wm_set_logits_processors")
+        self._lp_engine = self._handle.value if procs is not None else None
 
     def generate_from_pcm(self, pcm: Union[np.ndarray, torch.Tensor], language: Optional[str] = None,
                           task: Optional[str] = None, temperature=None, sampling_rate: int = SAMPLE_RATE,
@@ -571,6 +613,7 @@ class WhisperMedusaModel:
         ``return_token_timestamps`` as in ``generate``, with the clip's frame count (after resampling) as the attention
         mask's."""
         self._require_engine()
+        self._logits_processors(kwargs)
         n16 = (int(torch.as_tensor(pcm).numel()) if _rate(sampling_rate) == SAMPLE_RATE
                else resampled_length(int(torch.as_tensor(pcm).numel()), _rate(sampling_rate), SAMPLE_RATE))
         ts = (self._timestamp_request(None, task, self.pcm_num_frames(n16), time_precision)
@@ -637,6 +680,7 @@ class WhisperMedusaModel:
         no_speech = ((float(no_speech_threshold), float(logprob_threshold))
                      if no_speech_rule(no_speech_threshold, logprob_threshold) else None)
         self._check_unsupported(temperature, None, generate_kwargs)
+        self._logits_processors(generate_kwargs)
         if return_token_timestamps:
             self._timestamp_request(None, task, None, time_precision)
             generate_kwargs["time_precision"] = float(time_precision)
@@ -737,6 +781,9 @@ class WhisperMedusaModel:
         # generate() always runs the loop with temperature 1.0 => typical acceptance (model.py:1878-1881);
         # `medusa_temperature=0` selects the exact-match branch reachable through _medusa_greedy_search.
         t = kwargs.pop("medusa_temperature", 1.0)
+        procs = self._logits_processors(kwargs, g, prompt)
+        for k in _processors.KEYS:
+            kwargs.pop(k, None)
         max_length = kwargs.pop("max_length", None)
         if kwargs.get("max_new_tokens") is not None:         # HF: max_length = prompt + max_new_tokens
             max_length = len(prompt) + int(kwargs.pop("max_new_tokens"))
@@ -764,6 +811,7 @@ class WhisperMedusaModel:
             _check(lib, self._handle, lib.wm_set_alignment_heads(self._handle, arr, len(pairs) // 2),
                    "wm_set_alignment_heads")
             self._ts_engine = self._handle.value if pairs else None
+        self._push_logits_processors(procs)
         tr = self._run_loop(prompt, gp)
         self.last_trace = tr
         self._last_medusa_temperature = float(gp.temperature)

@@ -140,6 +140,7 @@ class StreamGroup:
         lead = self.models[0]
         lead._check_unsupported(kwargs.get("temperature"), None,
                                 {k: v for k, v in kwargs.items() if k not in ("language", "task", "temperature", "no_speech")})
+        lead._logits_processors(kwargs)
         if timed:
             lead._timestamp_request(None, kwargs.get("task"), None, time_precision)
             kwargs["time_precision"] = float(time_precision)
