@@ -111,6 +111,22 @@ int wm_set_suppress(wm_handle* h, const int32_t* suppress_ids, int32_t n_suppres
 int wm_set_logits_processors(wm_handle* h, const int32_t* seq_tokens, const int32_t* seq_offsets,
                              const float* seq_values, int32_t n_seqs, int32_t no_repeat_ngram_size,
                              int32_t eos_min_length);
+/* Sampled attempt of temperature fallback for the next wm_generate calls (until the next call of this function):
+ * temperature > 0 samples every emitted token from softmax(processed row / temperature) over the row's top-k set (all
+ * entries >= the k-th largest, ties kept; top_k = 0 or >= vocab_size: the whole row), by Gumbel-max with counter-based
+ * noise: the token at position n (index in the sequence, prompt included) is argmax_j(processed_j / T + g), with
+ * g = -log(-log u) from word j % 4 of Philox4x32-10(key = {seed_lo, seed_hi}, counter = {j / 4, n, window, attempt})
+ * (wm_sample_noise).  Speculation is kept: head rows propose their argmax and a candidate is accepted when it equals
+ * the verify row's sampled choice, so the tokens are those of a one-token-at-a-time Gumbel-max decode.  The loop's
+ * WmGenParams temperature must be 0 (exact-match acceptance).  Chains of medusa_choices only (wm_generate refuses a
+ * tree: WM_ERR_UNSUPPORTED).  top_k in 1 .. 64 or 0 (or >= vocab_size); other values WM_ERR_UNSUPPORTED; a negative
+ * or non-finite temperature WM_ERR_INVALID.  temperature = 0: sampling off (the default). */
+int wm_set_sampling(wm_handle* h, float temperature, int32_t top_k, uint32_t seed_lo, uint32_t seed_hi, uint32_t window,
+                    uint32_t attempt);
+/* The device's noise g of positions n, tokens j0 .. j0 + count - 1 under the given seed, window and attempt, as the
+ * sampled loop computes it (a test hook). */
+int wm_sample_noise(wm_handle* h, uint32_t seed_lo, uint32_t seed_hi, uint32_t window, uint32_t attempt, int32_t n,
+                    int32_t j0, int32_t count, float* out);
 
 /* ---- frontend + encoder (HF feature_extraction_whisper.py:135-164; modeling_whisper.py:593-647;
  *      cross-attention K/V projection :325-336) ------------------------------------------- */
@@ -213,7 +229,8 @@ int wm_last_logits(wm_handle* h, int32_t which, float* out);
  * cand = token of every node; row_argmax = argmax of every processed verify row; row_pc[n] (n >= 1) = probability of
  * node n's token in the temperature-scaled posterior of its parent row; row_thr[r] = min(posterior_threshold,
  * posterior_alpha * exp(-entropy)) of row r; *path_node = tree only: the node at depth accept of the best path.
- * row_pc / row_thr are not written at temperature 0; entries beyond the rows the step used are stale.  Any output may
+ * row_pc / row_thr are not written at temperature 0; entries beyond the rows the step used are stale.  In a sampled
+ * attempt (wm_set_sampling) row_argmax[r] of rows r < K is the row's sampled (perturbed) choice.  Any output may
  * be NULL.  WM_ERR_STATE unless the last call that ran the decode loop was a completed wm_generate (wm_forward also
  * rewrites the loop state). */
 int wm_last_accept(wm_handle* h, int32_t* cand, int32_t* row_argmax, float* row_pc, float* row_thr, int32_t* path_node);

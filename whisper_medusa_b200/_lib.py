@@ -62,6 +62,9 @@ SYMBOLS = {
     "wm_set_alignment_heads": (C.c_int, [C.c_void_p, _P(C.c_int32), C.c_int32]),
     "wm_set_logits_processors": (C.c_int, [C.c_void_p, _P(C.c_int32), _P(C.c_int32), _P(C.c_float), C.c_int32,
                                            C.c_int32, C.c_int32]),
+    "wm_set_sampling": (C.c_int, [C.c_void_p, C.c_float, C.c_int32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32]),
+    "wm_sample_noise": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_int32, C.c_int32,
+                                  C.c_int32, _P(C.c_float)]),
     "wm_token_timestamps": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_double, _P(C.c_float),
                                       _P(C.c_float), _P(C.c_int32)]),
     "wm_token_timestamps_from_probs": (C.c_int, [C.c_void_p, _P(C.c_float), C.c_int32, C.c_int32, C.c_int32, C.c_int32,

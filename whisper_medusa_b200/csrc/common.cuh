@@ -21,6 +21,8 @@ namespace wm {
 // most WM_MAX_T nodes, WM_TREE_MAX_CAND root-to-leaf paths and WM_TREE_MAX_TOPK candidates per head.
 #define WM_TREE_MAX_CAND 32
 #define WM_TREE_MAX_TOPK 4
+// largest top_k of a sampled attempt other than 0 (the whole row); HF's default is 50
+#define WM_SMP_MAX_TOPK 64
 struct DecTree {
   int n_tree, n_cand;
   int depth[16];        // medusa_position_ids: level of the node
@@ -243,6 +245,15 @@ struct DecState {
   // 32-bit words so that DecState keeps its 4-byte alignment (with an 8-byte member the loop kernels compile to
   // different register allocations).
   unsigned int adj_lo, adj_hi;
+  // sampled attempt of temperature fallback (wm_set_sampling; smp_on = 0: off, the loop chooses argmaxes).  Gumbel-max
+  // with counter-based noise (sample_gumbel): the base row of the tail and verify rows 0 .. K-1 choose
+  // argmax_j (processed_j / smp_temp + g(position, j)) over their top-k set {j : processed_j >= tau}; smp_topk = 0: the
+  // whole row.  The seed is two 32-bit words for the same reason as adj.
+  int smp_on, smp_topk;
+  float smp_temp;
+  unsigned int smp_key[2], smp_window, smp_attempt;
+  float tail_tau;                // tau of the tail's base row (-inf: the whole row), read by the scoring kernel
+  float row_tau[WM_MAX_T];       // tau of verify row r of the last accept step
 };
 __host__ __device__ __forceinline__ const float* dec_state_adj(const DecState* st) {
   return reinterpret_cast<const float*>(((unsigned long long)st->adj_hi << 32) | st->adj_lo);
@@ -269,6 +280,30 @@ __device__ __forceinline__ float processed_logit(const float* row, int j, const 
   return v;
 }
 
+// Philox4x32-10 (Salmon et al., "Parallel random numbers: as easy as 1, 2, 3", SC 2011): counter c, key k.
+__host__ __device__ __forceinline__ uint4 philox4x32_10(uint4 c, unsigned int k0, unsigned int k1) {
+#pragma unroll
+  for (int i = 0; i < 10; ++i) {
+    if (i) { k0 += 0x9E3779B9u; k1 += 0xBB67AE85u; }
+    const unsigned long long p0 = 0xD2511F53ull * c.x, p1 = 0xCD9E8D57ull * c.z;
+    c = make_uint4((unsigned int)(p1 >> 32) ^ c.y ^ k0, (unsigned int)p1, (unsigned int)(p0 >> 32) ^ c.w ^ k1,
+                   (unsigned int)p0);
+  }
+  return c;
+}
+// Gumbel noise of token j at position n (the index in DecState::ids the chosen token is written to) of a sampled
+// attempt: word j % 4 of Philox4x32-10(counter (j / 4, n, window, attempt), key = the seed's words) -> x,
+// u = ((x >> 8) + 0.5) 2^-24 in (0, 1), g = -log(-log u).  u and the logarithms are evaluated in double (u is exact
+// there; in fp32 the upper half of the range would round), and g is rounded once to fp32.
+__host__ __device__ __forceinline__ float sample_gumbel(const unsigned int key[2], unsigned int window,
+                                                        unsigned int attempt, int n, int j) {
+  const uint4 x = philox4x32_10(make_uint4((unsigned int)j >> 2, (unsigned int)n, window, attempt), key[0], key[1]);
+  const int w = j & 3;
+  const unsigned int b = w == 0 ? x.x : w == 1 ? x.y : w == 2 ? x.z : x.w;
+  const double u = ((double)(b >> 8) + 0.5) * (1.0 / 16777216.0);
+  return (float)(-log(-log(u)));
+}
+
 struct alignas(16) DecModel {   // (copied to shared memory in 16-byte pieces by the ring kernel)
   int d, H, ffn, V, S, S_pad;
   int n_layers;      // decoder layers (without the medusa block)
@@ -278,6 +313,7 @@ struct alignas(16) DecModel {   // (copied to shared memory in 16-byte pieces by
   int has_tree;      // 1 => branching choices: `tree` describes the candidate tree
   const DecTree* tree;
   float* topk_part;  // [WM_MAX_T rows][32 segments][WM_TREE_MAX_TOPK]{value, index}: per-segment top-k of the tail scan
+                     // (sampled attempts, which never have a tree: [WM_SMP_MAX_TOPK] entries per row and segment)
   DecLayer layers[WM_MAX_DEC_LAYERS];
   const __half* embed;   // [V, d] (also proj_out)
   const float* pos;      // [max_target_positions, d]

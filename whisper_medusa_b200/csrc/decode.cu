@@ -1076,6 +1076,156 @@ __device__ __noinline__ void stage_select2_rows(const DecModel* m, int cta, int 
   }
 }
 
+// Sampled attempt (DecState smp_on).  The rows whose choice decides an emitted token -- the tail's base row 0 (position
+// L) and verify rows r < K (position L + r + 1) -- store per segment either the perturbed maximum of
+// processed / T + g(position, j) (smp_topk = 0) or the segment's first min(k, finite entries) entries in (value desc,
+// index asc) order, their count and whether the segment has more entries equal to the last one (sel_part {max, argmax,
+// count, flag}).  The other rows keep the plain argmax (exact-match acceptance: the loop's temperature is 0).
+template <bool ADJ>
+__device__ __noinline__ void stage_select1_smp_rows(const DecModel* m, int mode, int cta, int ncta, unsigned char* smem_raw) {
+  const DecState* st = m->st;
+  const int V = m->V, K = m->K;
+  float* s_val = reinterpret_cast<float*>(smem_raw);
+  int* s_idx = reinterpret_cast<int*>(s_val + 32);
+  const int L = st->L;
+  const bool begin_on = (L == st->begin_index);
+  const float pen = m->pen_tab[L];
+  const int eos = st->eos;
+  const float* adj = ADJ ? dec_state_adj(st) : nullptr;
+  const float* logits = (mode == MODE_A) ? m->logits_a : m->logits_b;
+  const int nseg = select_nseg(m, ncta);
+  const int seglen = (V + nseg - 1) / nseg;
+  const int n_rows = (mode == MODE_A) ? K + 1 : m->n_tree;
+  const int kk = st->smp_topk;
+  const float temp = st->smp_temp;
+  for (int item = cta; item < n_rows * nseg; item += ncta) {
+    const int r = item / nseg, sg = item - r * nseg;
+    const int j0 = sg * seglen, j1 = min(V, j0 + seglen);
+    const float* row = logits + (size_t)r * V;
+    const bool sampled = (mode == MODE_A) ? r == 0 : r < K;
+    const bool perturb = sampled && kk == 0;
+    const int n = (mode == MODE_A) ? L : L + r + 1;
+    float bv = -INFINITY;
+    int bi = 0x7fffffff;
+    for (int j = j0 + threadIdx.x; j < j1; j += WM_DEC_THREADS) {
+      float v = processed_logit<ADJ>(row, j, m->tok_mask, begin_on, eos, pen, adj);
+      if (perturb) v = __fadd_rn(__fdiv_rn(v, temp), sample_gumbel(st->smp_key, st->smp_window, st->smp_attempt, n, j));
+      if (v > bv) { bv = v; bi = j; }
+    }
+    block_argmax(bv, bi, s_val, s_idx);
+    float* o = m->sel_part + ((size_t)r * WM_SEL_MAXSEG + sg) * 4;
+    if (!sampled || perturb) {
+      if (threadIdx.x == 0) { o[0] = bv; o[1] = __int_as_float(bi); o[2] = 0.f; }
+      continue;
+    }
+    // top-k list: one block-wide selection round per rank, as the tree's candidates (finite values only)
+    float* tp = m->topk_part + ((size_t)r * WM_SEL_MAXSEG + sg) * WM_SMP_MAX_TOPK * 2;
+    float pv = bv;
+    int pi = bi, cnt = (bi != 0x7fffffff) ? 1 : 0;
+    if (threadIdx.x == 0) { tp[0] = pv; tp[1] = __int_as_float(pi); }
+    while (cnt > 0 && cnt < kk) {
+      float cv = -INFINITY;
+      int ci = 0x7fffffff;
+      for (int j = j0 + threadIdx.x; j < j1; j += WM_DEC_THREADS) {
+        const float v = processed_logit<ADJ>(row, j, m->tok_mask, begin_on, eos, pen, adj);
+        if (ranks_after(v, j, pv, pi) && (v > cv)) { cv = v; ci = j; }
+      }
+      block_argmax(cv, ci, s_val, s_idx);
+      if (ci == 0x7fffffff) break;   // (uniform)
+      pv = cv; pi = ci;
+      if (threadIdx.x == 0) { tp[2 * cnt] = pv; tp[2 * cnt + 1] = __int_as_float(pi); }
+      ++cnt;
+    }
+    // a full list may leave out entries equal to its last value: the fold then rescans the segment if that value is tau
+    float more = 0.f;
+    if (cnt == kk)
+      for (int j = pi + 1 + threadIdx.x; j < j1; j += WM_DEC_THREADS)
+        if (processed_logit<ADJ>(row, j, m->tok_mask, begin_on, eos, pen, adj) == pv) more = 1.f;
+    more = block_sum(more, s_val);
+    if (threadIdx.x == 0) { o[0] = bv; o[1] = __int_as_float(bi); o[2] = __int_as_float(cnt); o[3] = __int_as_float(more > 0.f ? 1 : 0); }
+  }
+}
+__device__ __noinline__ void stage_select1_smp(const DecModel* m, int mode, int cta, int ncta, unsigned char* smem_raw) {
+  if (dec_state_adj(m->st)) stage_select1_smp_rows<true>(m, mode, cta, ncta, smem_raw);
+  else stage_select1_smp_rows<false>(m, mode, cta, ncta, smem_raw);
+}
+
+// Fold of sampled row r of `mode` (warp-cooperative, lane = segment; results uniform): the choice at position n, and tau,
+// the k-th largest processed value of the row (-inf = the whole row).  tau is the k-th pop of a merge of the sorted
+// segment lists; the choice is the perturbed maximum over every entry >= tau (ties on the sum: lowest index).
+__device__ __noinline__ void smp_fold(const DecModel* m, int mode, int r, int nseg, int n, int& idx, float& tau) {
+  const DecState* st = m->st;
+  const int kk = st->smp_topk;
+  if (kk == 0) {
+    float M, Z, ent;
+    select_fold(m, r, nseg, 1.0f, M, idx, Z, ent);
+    tau = -INFINITY;
+    return;
+  }
+  const int lane = threadIdx.x & 31;
+  const float2 none = make_float2(-INFINITY, __int_as_float(0x7fffffff));
+  int cnt = 0, flag = 0;
+  if (lane < nseg) {
+    const float4 q = __ldcg(reinterpret_cast<const float4*>(m->sel_part + (size_t)r * WM_SEL_MAXSEG * 4) + lane);
+    cnt = __float_as_int(q.z);
+    flag = __float_as_int(q.w);
+  }
+  const float* tp = m->topk_part + ((size_t)r * WM_SEL_MAXSEG + lane) * WM_SMP_MAX_TOPK * 2;
+  int p = 0;
+  float2 cur = cnt > 0 ? ldcg_f2(tp) : none, nxt = cnt > 1 ? ldcg_f2(tp + 2) : none;
+  tau = -INFINITY;
+  for (int q = 0; q < kk; ++q) {
+    float bv = cur.x;
+    int bi = __float_as_int(cur.y);
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      const float ov = __shfl_xor_sync(0xffffffffu, bv, o);
+      const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
+      if (ov > bv || (ov == bv && oi < bi)) { bv = ov; bi = oi; }
+    }
+    if (bi == 0x7fffffff) { tau = -INFINITY; break; }   // fewer than k finite values: the whole row (uniform)
+    tau = bv;
+    if (__float_as_int(cur.y) == bi) {                  // (indices are unique: one lane pops)
+      ++p;
+      cur = nxt;
+      nxt = (p + 1 < cnt) ? ldcg_f2(tp + 2 * (p + 1)) : none;
+    }
+  }
+  const float temp = st->smp_temp;
+  float best = -INFINITY;
+  int bidx = 0x7fffffff;
+  auto offer = [&](float v, int j) {
+    const float s = __fadd_rn(__fdiv_rn(v, temp), sample_gumbel(st->smp_key, st->smp_window, st->smp_attempt, n, j));
+    if (s > best || (s == best && j < bidx)) { best = s; bidx = j; }
+  };
+  float2 last = none;
+  for (int e = 0; e < cnt; ++e) {
+    last = ldcg_f2(tp + 2 * e);
+    if (!(last.x >= tau)) break;
+    offer(last.x, __float_as_int(last.y));
+  }
+  if (flag && cnt == kk && last.x == tau) {   // entries equal to tau beyond the segment's full list
+    const int V = m->V, seglen = (V + nseg - 1) / nseg, j1 = min(V, (lane + 1) * seglen);
+    const int L = st->L;
+    const bool begin_on = (L == st->begin_index);
+    const float pen = m->pen_tab[L];
+    const float* adj = dec_state_adj(st);
+    const float* row = ((mode == MODE_A) ? m->logits_a : m->logits_b) + (size_t)r * V;
+    for (int j = __float_as_int(last.y) + 1; j < j1; ++j) {
+      const float v = adj ? processed_logit<true>(row, j, m->tok_mask, begin_on, st->eos, pen, adj)
+                          : processed_logit<false>(row, j, m->tok_mask, begin_on, st->eos, pen, nullptr);
+      if (v == tau) offer(v, j);
+    }
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    const float ov = __shfl_xor_sync(0xffffffffu, best, o);
+    const int oi = __shfl_xor_sync(0xffffffffu, bidx, o);
+    if (ov > best || (ov == best && oi < bidx)) { best = ov; bidx = oi; }
+  }
+  idx = bidx;
+}
+
 // The variant with the logits-processor term, or without it, chosen by the uniform DecState adj (on / off for the whole
 // call): the stage and persistent kernels.  The ring kernel is instantiated with and without processors instead, so its
 // variant without them is the same code as a build without processors.
@@ -1088,14 +1238,22 @@ __device__ __noinline__ void stage_select2(const DecModel* m, int cta, int ncta,
   else stage_select2_rows<false>(m, cta, ncta, smem_raw);
 }
 
-// tail: candidates = top-1 of every head row (generate_candidates, medusa_utils.py:446-457)
+// tail: candidates = top-1 of every head row (generate_candidates, medusa_utils.py:446-457); SMP (sampled attempt, chain
+// only): c0 is the sampled choice of the base row
+template <bool SMP = false>
 __device__ __noinline__ void stage_select_fin(const DecModel* m, int ncta) {
   DecState* st = m->st;
   const int nseg = select_nseg(m, ncta);
   if (!m->has_tree) {
     for (int r = threadIdx.x >> 5; r <= m->K; r += (WM_DEC_THREADS >> 5)) {   // warp per row
       float M, Z, ent; int idx;
-      select_fold(m, r, nseg, 1.0f, M, idx, Z, ent);
+      if (SMP && r == 0) {
+        float tau;
+        smp_fold(m, MODE_A, 0, nseg, st->L, idx, tau);
+        if ((threadIdx.x & 31) == 0) st->tail_tau = tau;
+      } else {
+        select_fold(m, r, nseg, 1.0f, M, idx, Z, ent);
+      }
       if ((threadIdx.x & 31) == 0) st->cand[r] = idx;
     }
     return;
@@ -1146,6 +1304,9 @@ __device__ __noinline__ void stage_select_fin(const DecModel* m, int ncta) {
 //   accept-0 iteration (second emitted token = argmax of the verify row, never seen by the
 //   decoder) a one-token sweep A is needed (`need_a`).
 // -----------------------------------------------------------------------------------------
+// SMP (sampled attempt): the choice of verify row r < K is the sampled one (smp_fold at position L + r + 1, its tau kept
+// for the scoring kernel); the loop's temperature is 0, so acceptance is the exact match with it
+template <bool SMP = false>
 __device__ __noinline__ void stage_accept(const DecModel* m, int ncta) {
   __shared__ int s_a;
   __shared__ int s_arg[WM_MAX_T];
@@ -1158,7 +1319,13 @@ __device__ __noinline__ void stage_accept(const DecModel* m, int ncta) {
   for (int r = threadIdx.x >> 5; r <= K; r += (WM_DEC_THREADS >> 5)) {   // warp per row
     const float temp = st->temperature;
     float M, Z, ent; int idx;
-    select_fold(m, r, nseg, temp > 0.f ? 1.0f / temp : 1.0f, M, idx, Z, ent);
+    if (SMP && r < K) {
+      float tau;
+      smp_fold(m, MODE_B, r, nseg, st->L + r + 1, idx, tau);
+      if (lane == 0) st->row_tau[r] = tau;
+    } else {
+      select_fold(m, r, nseg, temp > 0.f ? 1.0f / temp : 1.0f, M, idx, Z, ent);
+    }
     if (lane == 0) {
       st->row_argmax[r] = idx;
       s_arg[r] = idx;
@@ -1432,8 +1599,9 @@ __host__ __device__ GemmDesc make_gemm_desc(const DecModel* m, int stage, int mo
 
 // WITH_GEMM = false: the caller runs the GEMM stages itself (ring kernel) -- keeps stage_gemm out of
 // that kernel's code.  ADJ: the logits scans with (1) or without (0) the logits-processor term, or chosen at run time
-// from dec_state_adj (-1)
-template <bool WITH_GEMM = true, int ADJ = -1>
+// from dec_state_adj (-1).  SMP: the sampled scan and folds of a sampled attempt (DecState smp_on; the processor term is
+// then chosen at run time)
+template <bool WITH_GEMM = true, int ADJ = -1, bool SMP = false>
 __device__ void run_stage(const DecModel* m, int stage, int mode, int layer, int cta, int ncta, unsigned char* smem,
                           const PassGeom* gopt = nullptr, unsigned long long* pr = nullptr) {
   switch (stage) {
@@ -1444,16 +1612,26 @@ __device__ void run_stage(const DecModel* m, int stage, int mode, int layer, int
     case ST_COPY_HIDDEN: stage_copy_hidden_to_x(m, mode, cta, ncta, gopt); break;
     case ST_TAIL_SEED: stage_tail_seed(m, cta, ncta); break;
     case ST_SELECT1:
-      if (ADJ < 0) stage_select1(m, mode, cta, ncta, smem);
+      if (SMP) stage_select1_smp(m, mode, cta, ncta, smem);
+      else if (ADJ < 0) stage_select1(m, mode, cta, ncta, smem);
       else stage_select1_rows<(ADJ > 0)>(m, mode, cta, ncta, smem);
       break;
     case ST_SELECT2:
       if (ADJ < 0) stage_select2(m, cta, ncta, smem);
       else stage_select2_rows<(ADJ > 0)>(m, cta, ncta, smem);
       break;
-    case ST_SELECT_FIN: if (cta == 0) stage_select_fin(m, ncta); break;
+    case ST_SELECT_FIN:
+      if (cta == 0) {
+        if (SMP) stage_select_fin<true>(m, ncta);
+        else stage_select_fin(m, ncta);
+      }
+      break;
     case ST_ACCEPT:
-      if (cta == 0) { if (m->has_tree) stage_accept_tree(m, ncta); else stage_accept(m, ncta); }
+      if (cta == 0) {
+        if (m->has_tree) stage_accept_tree(m, ncta);
+        else if (SMP) stage_accept<true>(m, ncta);
+        else stage_accept(m, ncta);
+      }
       break;
     case ST_KV_COMPACT: if (m->has_tree) stage_kv_compact(m, cta, ncta); break;
     default:
@@ -1497,15 +1675,16 @@ __host__ __device__ void seq_verify(int n_layers, int has_block, F&& f) {
 }
 
 // -----------------------------------------------------------------------------------------
-// mode 0: one kernel per stage (captured into CUDA graphs by the host)
+// mode 0: one kernel per stage (captured into CUDA graphs by the host); SMP: the variant of sampled attempts
 // -----------------------------------------------------------------------------------------
+template <bool SMP = false>
 __global__ void __launch_bounds__(WM_DEC_THREADS, 1)
 dec_stage_kernel(const DecModel* __restrict__ m, int stage, int mode, int layer, int phase) {
   extern __shared__ __align__(128) unsigned char smem[];
   const DecState* st = m->st;
   if (st->done) return;
   if (phase == PH_SWEEP_A && !st->need_a) return;
-  run_stage(m, stage, mode, layer, blockIdx.x, gridDim.x, smem);
+  run_stage<true, -1, SMP>(m, stage, mode, layer, blockIdx.x, gridDim.x, smem);
 }
 
 // -----------------------------------------------------------------------------------------
@@ -1549,6 +1728,7 @@ __device__ __forceinline__ void grid_barrier(unsigned int* bar, unsigned int& ep
   epoch = grid_barrier_step<true>(bar, epoch, ncta);
 }
 
+template <bool SMP = false>
 __global__ void __launch_bounds__(WM_DEC_THREADS, 1)
 dec_iteration_kernel(const DecModel* __restrict__ m) {
   extern __shared__ __align__(128) unsigned char smem[];
@@ -1561,7 +1741,7 @@ dec_iteration_kernel(const DecModel* __restrict__ m) {
   unsigned int* bar = m->bar;
   const int cta = blockIdx.x, ncta = gridDim.x;
   auto run = [&](int stage, int mode, int layer) {
-    run_stage(m, stage, mode, layer, cta, ncta, smem);
+    run_stage<true, -1, SMP>(m, stage, mode, layer, cta, ncta, smem);
     grid_barrier(bar, epoch, ncta);
   };
   if (need_a) seq_sweep(m->n_layers, m->has_block, MODE_A, run);
@@ -1914,11 +2094,13 @@ cudaError_t dec_relayout_cross_kv(const __half* kv, __half* ck, __half* cv, int 
   return cudaGetLastError();
 }
 
-// profile: the stage-timeline variant (processors chosen at run time); lp: the variant with logits processors
-static void* ring_kernel_fn(int d, bool profile, bool lp = false) {
+// profile: the stage-timeline variant (processors chosen at run time); smp: the variant of sampled attempts (processors
+// chosen at run time); lp: the variant with logits processors
+static void* ring_kernel_fn(int d, bool profile, bool lp = false, bool smp = false) {
   switch (d) {
 #define WM_CASE(DD)                                                                                                          \
   case DD:                                                                                                                   \
+    if (smp) return profile ? (void*)dec_iteration_ring_kernel<DD, true, false, true> : (void*)dec_iteration_ring_kernel<DD, false, false, true>; \
     return profile ? (void*)dec_iteration_ring_kernel<DD, true, false>                                                      \
                    : lp ? (void*)dec_iteration_ring_kernel<DD, false, true> : (void*)dec_iteration_ring_kernel<DD, false, false>;
     WM_RING_WIDTHS(WM_CASE)
@@ -1929,7 +2111,7 @@ static void* ring_kernel_fn(int d, bool profile, bool lp = false) {
 
 // Cooperative launch (the grid barrier needs every CTA resident), as clusters of hi.cluster CTAs along x.
 cudaError_t dec_launch_iteration_ring(const DecModel* dm, const DecHostInfo& hi, bool profile, cudaStream_t s) {
-  void* fn = ring_kernel_fn(hi.d, profile, hi.lp != 0);
+  void* fn = ring_kernel_fn(hi.d, profile, hi.lp != 0, hi.smp != 0);
   if (!fn) return cudaErrorInvalidValue;
   void* args[] = {(void*)&dm};
   cudaLaunchAttribute attr[2];
@@ -1983,10 +2165,12 @@ size_t dec_smem_bytes(int d, int ffn) {
 }
 
 cudaError_t dec_configure(int d, size_t smem, size_t smem_ring) {
-  cudaError_t e = cudaFuncSetAttribute(dec_stage_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  if (e != cudaSuccess) return e;
-  e = cudaFuncSetAttribute(dec_iteration_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  if (e != cudaSuccess) return e;
+  for (const void* fn : {(const void*)dec_stage_kernel<false>, (const void*)dec_stage_kernel<true>,
+                         (const void*)dec_iteration_kernel<false>, (const void*)dec_iteration_kernel<true>}) {
+    const cudaError_t e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return e;
+  }
+  cudaError_t e;
   if (smem_ring == 0) return cudaSuccess;   // decoder width without a ring instantiation: persistent mode refuses to run
   switch (d) {
 #define WM_CASE(DD)                                                                                                          \
@@ -1994,6 +2178,10 @@ cudaError_t dec_configure(int d, size_t smem, size_t smem_ring) {
     e = cudaFuncSetAttribute(dec_iteration_ring_kernel<DD, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_ring); \
     if (e != cudaSuccess) return e;                                                                                          \
     e = cudaFuncSetAttribute(dec_iteration_ring_kernel<DD, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_ring); \
+    if (e != cudaSuccess) return e;                                                                                          \
+    e = cudaFuncSetAttribute(dec_iteration_ring_kernel<DD, false, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_ring); \
+    if (e != cudaSuccess) return e;                                                                                          \
+    e = cudaFuncSetAttribute(dec_iteration_ring_kernel<DD, true, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_ring); \
     if (e != cudaSuccess) return e;                                                                                          \
     return cudaFuncSetAttribute(dec_iteration_ring_kernel<DD, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_ring);
     WM_RING_WIDTHS(WM_CASE)
@@ -2025,7 +2213,9 @@ cudaError_t dec_enqueue_phase(const DecModel* dm, const DecHostInfo& hi, int pha
   auto launch = [&](int stage, int mode, int layer) {
     const int rows = pass_geom(mode, T, 0, hi.n_tree).T;   // (sweep A over T rows: L = T, kv_len = 0)
     const int grid = stage_grid(stage, rows, hi.n_sm, hi.H, hi.K);
-    dec_stage_kernel<<<grid, WM_DEC_THREADS, hi.smem, s>>>(dm, stage, mode, layer, phase);
+    // (sweep A has no logits scan: its graphs, shared by every call, keep the kernel without sampling)
+    if (hi.smp && phase != PH_SWEEP_A) dec_stage_kernel<true><<<grid, WM_DEC_THREADS, hi.smem, s>>>(dm, stage, mode, layer, phase);
+    else dec_stage_kernel<false><<<grid, WM_DEC_THREADS, hi.smem, s>>>(dm, stage, mode, layer, phase);
     if (n_launch) ++*n_launch;
   };
   if (phase == PH_SWEEP_A) seq_sweep(hi.n_layers, hi.has_block, MODE_A, launch);
@@ -2034,9 +2224,23 @@ cudaError_t dec_enqueue_phase(const DecModel* dm, const DecHostInfo& hi, int pha
   return cudaGetLastError();
 }
 
+__global__ void sample_noise_kernel(uint2 key, unsigned int window, unsigned int attempt, int n, int j0, int count,
+                                    float* __restrict__ out) {
+  const unsigned int k[2] = {key.x, key.y};
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < count; i += gridDim.x * blockDim.x)
+    out[i] = sample_gumbel(k, window, attempt, n, j0 + i);
+}
+cudaError_t dec_launch_sample_noise(const unsigned int key[2], unsigned int window, unsigned int attempt, int n, int j0,
+                                    int count, float* out, cudaStream_t s) {
+  sample_noise_kernel<<<std::min(1024, (count + 255) / 256), 256, 0, s>>>(make_uint2(key[0], key[1]), window, attempt, n,
+                                                                          j0, count, out);
+  return cudaGetLastError();
+}
+
 cudaError_t dec_launch_iteration(const DecModel* dm, const DecHostInfo& hi, cudaStream_t s) {
   void* args[] = {(void*)&dm};
-  return cudaLaunchCooperativeKernel((void*)dec_iteration_kernel, dim3(hi.n_sm), dim3(WM_DEC_THREADS), args, hi.smem, s);
+  const void* fn = hi.smp ? (const void*)dec_iteration_kernel<true> : (const void*)dec_iteration_kernel<false>;
+  return cudaLaunchCooperativeKernel(fn, dim3(hi.n_sm), dim3(WM_DEC_THREADS), args, hi.smem, s);
 }
 
 }  // namespace wm

@@ -795,8 +795,9 @@ __device__ __forceinline__ void stage_self_attn_ring(RingState& rs, unsigned cha
   }
 }
 
-// LP: the logits scans with the logits-processor term (dec_state_adj); the profiling variant chooses at run time
-template <int D, bool PROF, bool LP>
+// LP: the logits scans with the logits-processor term (dec_state_adj); SMP: a sampled attempt's scans and folds (DecState
+// smp_on; processors chosen at run time); the profiling variant chooses processors at run time
+template <int D, bool PROF, bool LP, bool SMP = false>
 __global__ void __launch_bounds__(WM_RING_THREADS, 1)
 dec_iteration_ring_kernel(const DecModel* __restrict__ gm) {
   using G = RingGeom<D>;
@@ -881,7 +882,8 @@ dec_iteration_ring_kernel(const DecModel* __restrict__ gm) {
     } else if (stage == ST_SELF_ATTN) {
       stage_self_attn_ring<D>(rs, smem, m, mode, sd->layer, cta, ncta, pgv, L0, kv0, pr);
     } else {
-      run_stage<false, PROF ? -1 : (LP ? 1 : 0)>(m, stage, mode, sd->layer, cta, ncta, smem + G::SCRATCH_OFF, &pgv, pr);
+      run_stage<false, (PROF || SMP) ? -1 : (LP ? 1 : 0), SMP>(m, stage, mode, sd->layer, cta, ncta,
+                                                                      smem + G::SCRATCH_OFF, &pgv, pr);
     }
     if (prof) pr[15] = global_timer_ns();
     if (fetch) reinterpret_cast<uint32_t*>(&s_desc[(ip + 1) & 1])[lane] = nxt_w;

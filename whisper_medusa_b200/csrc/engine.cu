@@ -72,8 +72,9 @@ struct wm_handle {
   DecHostInfo hi;
   std::map<int, cudaGraphExec_t> graph_a;  // sweep A, keyed by T
   cudaGraphExec_t graph_tail = nullptr, graph_b = nullptr;
+  cudaGraphExec_t graph_smp[2] = {nullptr, nullptr};   // tail / verify graphs of sampled attempts (their stage kernels)
   int64_t launches_a[WM_MAX_T + 1] = {0};
-  int64_t launches_tail = 0, launches_b = 0;
+  int64_t launches_tail = 0, launches_b = 0, launches_smp[2] = {0, 0};
   int decode_mode = 0;
   int enc_gemm_impl = 0;   // 0 = mma.sync kernel, 1 = wgmma/TMA kernel
   int enc_pdl = 1;         // encoder kernels launched with programmatic stream serialization (option "enc_pdl" = 0: plain launches)
@@ -130,6 +131,10 @@ struct wm_handle {
   // logits processors (wm_set_logits_processors); buffers allocated on first use
   int lp_on = 0;
   LogitsProcArgs lp{};          // device tables: base [V], adj [V], seq_tok / seq_off / seq_val (WM_LP_MAX_* entries)
+  // sampled attempt (wm_set_sampling): temperature 0 = off
+  float smp_temp = 0.f;
+  int smp_topk = 0;
+  unsigned int smp_key[2] = {0u, 0u}, smp_window = 0u, smp_attempt = 0u;
 };
 
 #define WM_TS_MAX_LIST 64   // alignment pairs per call (duplicates included)
@@ -338,7 +343,7 @@ extern "C" int wm_create(const wm_config* cfg, int device, wm_handle** out) {
   m.n_layers = c.dec_layers; m.has_block = c.medusa_block ? 1 : 0; m.K = c.medusa_num_heads;
   m.n_tree = c.medusa_num_heads + 1; m.has_tree = 0; m.tree = nullptr;
   CK(dalloc(&h->tree, 1));
-  CK(dalloc(&m.topk_part, (size_t)WM_MAX_T * 32 * WM_TREE_MAX_TOPK * 2));
+  CK(dalloc(&m.topk_part, (size_t)WM_MAX_T * 32 * std::max(WM_TREE_MAX_TOPK, WM_SMP_MAX_TOPK) * 2));
   CK(dalloc(&m.x, (size_t)WM_MAX_T * d));
   CK(dalloc(&m.xg, (size_t)WM_MAX_T * d));
   CK(dalloc(&m.q, (size_t)WM_MAX_T * d));
@@ -396,6 +401,8 @@ static void drop_graphs(wm_handle* h) {
   h->graph_a.clear();
   if (h->graph_b) { cudaGraphExecDestroy(h->graph_b); h->graph_b = nullptr; }
   if (h->graph_tail) { cudaGraphExecDestroy(h->graph_tail); h->graph_tail = nullptr; }
+  for (auto& g : h->graph_smp)
+    if (g) { cudaGraphExecDestroy(g); g = nullptr; }
 }
 
 extern "C" int wm_destroy(wm_handle* h) {
@@ -815,8 +822,10 @@ extern "C" int wm_encode_mel(wm_handle* h, const float* mel) {
 // decode loop
 // ---------------------------------------------------------------------------------------------
 static int get_graph(wm_handle* h, int phase, int T, cudaGraphExec_t* out, int64_t* n_launch) {
-  if (phase == 2 && h->graph_b) { *out = h->graph_b; *n_launch = h->launches_b; return WM_OK; }
-  if (phase == 1 && h->graph_tail) { *out = h->graph_tail; *n_launch = h->launches_tail; return WM_OK; }
+  const bool smp = h->hi.smp && phase >= 1;
+  if (smp && h->graph_smp[phase - 1]) { *out = h->graph_smp[phase - 1]; *n_launch = h->launches_smp[phase - 1]; return WM_OK; }
+  if (!smp && phase == 2 && h->graph_b) { *out = h->graph_b; *n_launch = h->launches_b; return WM_OK; }
+  if (!smp && phase == 1 && h->graph_tail) { *out = h->graph_tail; *n_launch = h->launches_tail; return WM_OK; }
   if (phase == 0) {
     auto it = h->graph_a.find(T);
     if (it != h->graph_a.end()) { *out = it->second; *n_launch = h->launches_a[T]; return WM_OK; }
@@ -831,7 +840,8 @@ static int get_graph(wm_handle* h, int phase, int T, cudaGraphExec_t* out, int64
   cudaGraphExec_t ge;
   CK(cudaGraphInstantiate(&ge, g, 0));
   CK(cudaGraphDestroy(g));
-  if (phase == 2) { h->graph_b = ge; h->launches_b = nl; }
+  if (smp) { h->graph_smp[phase - 1] = ge; h->launches_smp[phase - 1] = nl; }
+  else if (phase == 2) { h->graph_b = ge; h->launches_b = nl; }
   else if (phase == 1) { h->graph_tail = ge; h->launches_tail = nl; }
   else { h->graph_a[T] = ge; h->launches_a[T] = nl; }
   *out = ge; *n_launch = nl;
@@ -886,6 +896,9 @@ extern "C" int wm_generate(wm_handle* h, const int32_t* prompt, int32_t n_prompt
   if (n_prompt < 1 || n_prompt + K + 2 > gp->max_length) return fail(h, WM_ERR_INVALID, "prompt length must be in [1, max_length - K - 2)");
   if (gp->max_length > h->cfg.max_target_positions) return fail(h, WM_ERR_INVALID, "max_length exceeds max_target_positions");
   if (gp->temperature < 0.f) return fail(h, WM_ERR_INVALID, "temperature must be >= 0");
+  if (h->smp_temp > 0.f && h->hm.has_tree) return fail(h, WM_ERR_UNSUPPORTED, "sampling needs a chain of medusa_choices");
+  if (h->smp_temp > 0.f && gp->temperature != 0.f)
+    return fail(h, WM_ERR_INVALID, "a sampled attempt runs the loop at temperature 0 (exact-match acceptance)");
   for (int i = 0; i < n_prompt; ++i)
     if (prompt[i] < 0 || prompt[i] >= h->cfg.vocab_size) return fail(h, WM_ERR_INVALID, "prompt id out of range");
   // the no-speech row must be computed by the first real iteration: not in a prefill chunk (the first
@@ -935,6 +948,10 @@ extern "C" int wm_generate(wm_handle* h, const int32_t* prompt, int32_t n_prompt
     hs.post_alpha = gp->posterior_alpha;
     hs.tree_attn = (h->hm.has_tree && gp->tree_attention) ? 1 : 0;
     dec_state_set_adj(&hs, h->lp_on ? h->lp.adj : nullptr);
+    hs.smp_on = h->smp_temp > 0.f ? 1 : 0;
+    hs.smp_temp = h->smp_temp; hs.smp_topk = h->smp_topk;
+    hs.smp_key[0] = h->smp_key[0]; hs.smp_key[1] = h->smp_key[1];
+    hs.smp_window = h->smp_window; hs.smp_attempt = h->smp_attempt;
     for (int i = 0; i < n_prompt; ++i) hs.ids[i] = prompt[i];
     // reference stop rule evaluated before the first iteration is never true for sane inputs; the
     // loop always runs at least once (model.py:635).
@@ -952,9 +969,11 @@ extern "C" int wm_generate(wm_handle* h, const int32_t* prompt, int32_t n_prompt
   sa.want_lp = score_bits & 1; sa.want_rows = (score_bits >> 1) & 1;
   sa.state = h->score_state; sa.part = h->score_part; sa.lp = h->score_lp; sa.rows = h->score_rows;
   sa.cap_rows = h->cfg.max_target_positions;
+  sa.tau = h->h_init->smp_on && h->smp_topk > 0;
   const int score_grid = dec_score_grid(h->n_cta, K);
   const bool lp_on = dec_state_adj(h->h_init) != nullptr;
   h->hi.lp = lp_on;   // (prefill launches only run sweep A: no logits scan)
+  h->hi.smp = h->h_init->smp_on;
   LogitsProcArgs la = h->lp;
   la.st = h->st;
   const int lp_grid = dec_logits_proc_grid(h->n_cta);
@@ -1163,6 +1182,37 @@ extern "C" int wm_set_logits_processors(wm_handle* h, const int32_t* seq_tokens,
   return WM_OK;
 }
 
+extern "C" int wm_set_sampling(wm_handle* h, float temperature, int32_t top_k, uint32_t seed_lo, uint32_t seed_hi,
+                               uint32_t window, uint32_t attempt) {
+  if (!h) return WM_ERR_INVALID;
+  if (!std::isfinite(temperature) || temperature < 0.f) return fail(h, WM_ERR_INVALID, "temperature must be finite and >= 0");
+  if (top_k < 0) return fail(h, WM_ERR_UNSUPPORTED, "top_k must be >= 0");
+  if (top_k >= h->cfg.vocab_size) top_k = 0;   // the whole row, as HF's min(top_k, vocab_size)
+  if (top_k > WM_SMP_MAX_TOPK) return fail(h, WM_ERR_UNSUPPORTED, "top_k must be at most 64 (or 0: the whole vocabulary)");
+  h->smp_temp = temperature;
+  h->smp_topk = top_k;
+  h->smp_key[0] = seed_lo; h->smp_key[1] = seed_hi;
+  h->smp_window = window; h->smp_attempt = attempt;
+  return WM_OK;
+}
+
+extern "C" int wm_sample_noise(wm_handle* h, uint32_t seed_lo, uint32_t seed_hi, uint32_t window, uint32_t attempt,
+                               int32_t n, int32_t j0, int32_t count, float* out) {
+  if (!h || !out || count < 0 || j0 < 0 || n < 0) return WM_ERR_INVALID;
+  if (h->device < 0) return fail(h, WM_ERR_STATE, "layout-only handle");
+  if (count == 0) return WM_OK;
+  CK(cudaSetDevice(h->device));
+  float* d = nullptr;
+  CK(dalloc(&d, (size_t)count));
+  const unsigned int key[2] = {seed_lo, seed_hi};
+  cudaError_t e = dec_launch_sample_noise(key, window, attempt, n, j0, count, d, h->stream);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(out, d, (size_t)count * sizeof(float), cudaMemcpyDeviceToHost, h->stream);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(h->stream);
+  cudaFree(d);
+  CK(e);
+  return WM_OK;
+}
+
 static int ts_probs_reserve(wm_handle* h, size_t elems) {
   if (elems <= h->ts_probs_cap) return WM_OK;
   if (h->ts_probs) CK(cudaFree(h->ts_probs));
@@ -1342,6 +1392,7 @@ extern "C" int wm_forward(wm_handle* h, const int32_t* ids, int32_t n_ids, float
   const size_t V = (size_t)h->cfg.vocab_size;
   h->st_from_generate = 0;   // the loop state is rewritten below
   h->hi.lp = 0;              // (no logits processors: the state below has no adj)
+  h->hi.smp = 0;
   {
     const int r = set_ts_capture(h, false);   // (the passes below must not overwrite the last wm_generate's captured
     if (r != WM_OK) return r;                  //  alignment rows, nor its no-speech row)

@@ -19,6 +19,7 @@ struct DecHostInfo {
   size_t smem_ring;
   int cluster = 1; // CTAs per cluster of the ring kernel (1 or 2, dec_ring_cluster_size)
   int lp = 0;      // 1: logits processors on for the iterations enqueued next (the ring kernel's variant with them)
+  int smp = 0;     // 1: a sampled attempt (wm_set_sampling): the ring kernel's variant with the sampled scans and folds
 };
 
 // ---- decode.cu ----
@@ -69,9 +70,14 @@ struct ScoreArgs {
   float* lp;               // [WM_MAX_POS + 32]: log-probability of the token at each position
   float* rows;             // [cap_rows][V]: processed verify row path[accept] of each iteration
   int cap_rows;
+  int tau;                 // 1: a sampled attempt with top-k: token rows are restricted to {v >= tau} (DecState tail_tau,
+                           // row_tau), as HF's log_softmax of the warped scores at temperature 1
 };
 int dec_score_grid(int n_cta, int K);
 cudaError_t dec_launch_scores(const ScoreArgs& a, int grid, cudaStream_t s);
+// Gumbel noise of a sampled attempt (sample_gumbel) at position n for tokens j0 .. j0 + count - 1 (wm_sample_noise)
+cudaError_t dec_launch_sample_noise(const unsigned int key[2], unsigned int window, unsigned int attempt, int n, int j0,
+                                    int count, float* out, cudaStream_t s);
 
 // ---- logits_proc.cu ----
 #define WM_LP_THREADS 256

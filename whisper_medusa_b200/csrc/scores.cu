@@ -11,6 +11,8 @@
 //   scores row of the iteration              <- verify row path[a] (the reference's next_token_logits)
 // log_softmax at temperature 1: fp32, max-subtracted, in WM_SCORE_NSEG vocabulary segments per row whose partials are
 // folded in segment order by the last CTA to arrive, so the result does not depend on the grid size.
+// TAU (a sampled attempt with top-k): a token row keeps only its top-k set {v >= tau} (DecState tail_tau for c0, row_tau
+// for verify rows), as HF's log_softmax of the warped scores times the temperature; the scores rows stay unrestricted.
 #include <algorithm>
 
 #include "common.cuh"
@@ -36,7 +38,7 @@ __device__ __forceinline__ int path_node(const DecState* st, const DecTree* tree
   return node;
 }
 
-template <bool ADJ>
+template <bool ADJ, bool TAU = false>
 __global__ void __launch_bounds__(WM_SCORE_THREADS) score_iteration_kernel(ScoreArgs p) {
   constexpr int NW = WM_SCORE_THREADS / 32;
   __shared__ float s_m[NW], s_s[NW];
@@ -67,6 +69,7 @@ __global__ void __launch_bounds__(WM_SCORE_THREADS) score_iteration_kernel(Score
       continue;
     }
     const float* row = (r == 0) ? p.logits_a : p.logits_b + (size_t)path_node(st, p.tree, a, r - 1) * V;
+    const float tau = TAU ? (r == 0 ? st->tail_tau : st->row_tau[r - 1]) : -INFINITY;
     if (threadIdx.x == 0) {   // the segment holding the row's token also records its processed logit for the fold
       const int tok = st->ids[L0 + r];
       if (tok >= j0 && tok < j1) p.part[(size_t)(WM_MAX_T + 1) * WM_SCORE_NSEG * 2 + r] = processed_logit<ADJ>(row, tok, p.tok_mask, begin_on, eos, pen, p.adj);
@@ -80,6 +83,7 @@ __global__ void __launch_bounds__(WM_SCORE_THREADS) score_iteration_kernel(Score
       for (int u = 0; u < WM_SCORE_UNROLL; ++u) {
         const int j = jb + u * WM_SCORE_THREADS;
         v[u] = j < j1 ? processed_logit<ADJ>(row, j, p.tok_mask, begin_on, eos, pen, p.adj) : -INFINITY;
+        if (TAU && v[u] < tau) v[u] = -INFINITY;
       }
 #pragma unroll
       for (int u = 0; u < WM_SCORE_UNROLL; ++u) {
@@ -136,7 +140,10 @@ __global__ void __launch_bounds__(WM_SCORE_THREADS) score_iteration_kernel(Score
 int dec_score_grid(int n_cta, int K) { return std::min(n_cta, (K + 2) * WM_SCORE_NSEG); }
 
 cudaError_t dec_launch_scores(const ScoreArgs& a, int grid, cudaStream_t s) {
-  if (a.adj) score_iteration_kernel<true><<<grid, WM_SCORE_THREADS, 0, s>>>(a);
+  if (a.tau) {
+    if (a.adj) score_iteration_kernel<true, true><<<grid, WM_SCORE_THREADS, 0, s>>>(a);
+    else score_iteration_kernel<false, true><<<grid, WM_SCORE_THREADS, 0, s>>>(a);
+  } else if (a.adj) score_iteration_kernel<true><<<grid, WM_SCORE_THREADS, 0, s>>>(a);
   else score_iteration_kernel<false><<<grid, WM_SCORE_THREADS, 0, s>>>(a);
   return cudaGetLastError();
 }

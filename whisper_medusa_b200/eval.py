@@ -19,7 +19,9 @@ scores (`metrics.py` restates jiwer 3.0.3, see there).  Differences, all on the 
   (the reference accepts at most 30 s).  The default 0 keeps the path above;
 * `--no-speech-threshold P --logprob-threshold L`: HF's no-speech rule.  Chunked mode passes both to `transcribe`
   (silent windows add no text); otherwise each clip's `generate` dict output is tested with the same rule
-  (`longform.skip_window`) and a silent clip's hypothesis is empty.
+  (`longform.skip_window`) and a silent clip's hypothesis is empty;
+* `--temperature 0,0.2,0.4,0.6,0.8,1 --compression-ratio-threshold 2.4 [--logprob-threshold L]`: temperature fallback,
+  passed to `transcribe` in chunked mode (refused without `--chunk-length-s`).
 """
 from __future__ import annotations
 
@@ -104,7 +106,8 @@ def evaluate_rows(rows: Iterable[Dict], transcribe: Callable[[np.ndarray, str], 
 def evaluate_model(model_name: str, data_path: str, out_file_path: str, language: str = "en",
                    regulation_start: float = 140, regulation_factor: float = 1.0, frontend: str = "engine",
                    device: str = "cuda:0", chunk_length_s: float = 0.0, no_speech_threshold: Optional[float] = None,
-                   logprob_threshold: Optional[float] = None):
+                   logprob_threshold: Optional[float] = None, temperature: Optional[Sequence[float]] = None,
+                   compression_ratio_threshold: Optional[float] = None):
     import pandas as pd
     import torch
     from transformers import WhisperProcessor
@@ -112,7 +115,12 @@ def evaluate_model(model_name: str, data_path: str, out_file_path: str, language
     from . import WhisperMedusaModel
     from .longform import no_speech_rule, skip_window
 
-    rule = no_speech_rule(no_speech_threshold, logprob_threshold)
+    if (temperature is not None or compression_ratio_threshold is not None) and chunk_length_s <= 0:
+        raise ValueError("--temperature / --compression-ratio-threshold (temperature fallback) need --chunk-length-s")
+    fallback = {} if temperature is None else {"temperature": tuple(temperature),
+                                               "compression_ratio_threshold": compression_ratio_threshold}
+    # (with a schedule, transcribe takes --logprob-threshold alone as a fallback threshold)
+    rule = no_speech_rule(no_speech_threshold, None if fallback and no_speech_threshold is None else logprob_threshold)
 
     data = pd.read_csv(data_path).fillna("")
     processor = WhisperProcessor.from_pretrained(model_name)
@@ -124,7 +132,7 @@ def evaluate_model(model_name: str, data_path: str, out_file_path: str, language
             x, sr = pcm
             out = model.transcribe(x, sampling_rate=sr, chunk_length_s=chunk_length_s, language=lang,
                                    exponential_decay_length_penalty=penalty, no_speech_threshold=no_speech_threshold,
-                                   logprob_threshold=logprob_threshold)
+                                   logprob_threshold=logprob_threshold, **fallback)
             return processor.decode(out[0], skip_special_tokens=True)
         ns = dict(return_dict_in_generate=True, output_no_speech_prob=True) if rule else {}
         if frontend == "hf":
@@ -167,11 +175,18 @@ def main(argv: Optional[Sequence[str]] = None):
                     help="skip a window / clip whose <|nospeech|> probability is above this (needs --logprob-threshold)")
     ap.add_argument("--logprob-threshold", type=float, default=None,
                     help="... and whose average token log-probability is below this")
+    ap.add_argument("--temperature", type=str, default=None,
+                    help="temperature-fallback schedule, comma-separated, first entry 0 (e.g. 0,0.2,0.4,0.6,0.8,1); "
+                         "--chunk-length-s mode")
+    ap.add_argument("--compression-ratio-threshold", type=float, default=None,
+                    help="decode a window again at the next temperature when its compression ratio is above this")
     args = ap.parse_args(argv)
     logging.basicConfig(format="%(asctime)s - %(name)s - %(levelname)s - %(message)s", level=logging.INFO)
     evaluate_model(args.model_name, args.data_path, args.out_file_path, args.language, args.regulation_start,
                    args.regulation_factor, args.frontend, args.device, args.chunk_length_s, args.no_speech_threshold,
-                   args.logprob_threshold)
+                   args.logprob_threshold,
+                   None if args.temperature is None else [float(v) for v in args.temperature.split(",")],
+                   args.compression_ratio_threshold)
 
 
 if __name__ == "__main__":

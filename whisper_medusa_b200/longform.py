@@ -19,11 +19,16 @@ recording's time axis, ``token_pairs`` turns its token times into ``(start, end)
 ``pairs`` is ``_find_longest_common_sequence(sequences, token_timestamp_sequences)``, whose match rule is stricter
 (equal ids whose times are in order), so its ids can differ from the untimed merge's.
 
+With a temperature schedule and ``compression_ratio_threshold`` / ``logprob_threshold``, a window is decoded again by
+sampling at the schedule's next temperature while its result needs fallback (``fallback_rule``, ``needs_fallback``:
+HF's ``generate_with_fallback`` and ``_need_fallback``).
+
 The CPU tests pin all of it to the installed transformers; the package does not import it.
 """
 from __future__ import annotations
 
 import math
+import zlib
 from typing import List, NamedTuple, Optional, Sequence, Tuple, Union
 
 import numpy as np
@@ -184,8 +189,8 @@ def no_speech_rule(no_speech_threshold, logprob_threshold) -> bool:
     """Check the no-speech arguments of ``transcribe``; True when windows are to be tested for silence.
 
     HF's rule needs both thresholds: ``no_speech_threshold`` alone raises ``ValueError`` (HF itself fails comparing
-    with ``None`` there).  ``logprob_threshold`` alone means temperature fallback, which greedy-only Medusa decoding
-    cannot do: ``NotImplementedError``.  Both must be finite numbers."""
+    with ``None`` there).  ``logprob_threshold`` alone means temperature fallback, which needs a temperature schedule
+    (``fallback_rule``; callers with one do not pass it here): ``NotImplementedError``.  Both must be finite numbers."""
     if no_speech_threshold is None and logprob_threshold is None:
         return False
     if logprob_threshold is None:
@@ -208,6 +213,83 @@ def skip_window(no_speech_prob: float, avg_logprob: float, no_speech_threshold: 
     return avg_logprob < logprob_threshold and no_speech_prob > no_speech_threshold
 
 
+# largest top_k of a sampled attempt other than 0 (the whole vocabulary): the engine's per-segment candidate lists
+MAX_TOP_K = 64
+
+
+class Fallback(NamedTuple):
+    """Temperature fallback of ``transcribe``: the schedule (first entry 0.0) and the thresholds (None = not tested)."""
+    temperatures: Tuple[float, ...]
+    compression_ratio_threshold: Optional[float]
+    logprob_threshold: Optional[float]
+    top_k: int                # 0 = the whole vocabulary
+
+
+def _finite(name: str, v) -> float:
+    if isinstance(v, bool) or not isinstance(v, (int, float, np.floating, np.integer)) or not math.isfinite(float(v)):
+        raise ValueError(f"{name} must be a finite float, got {v!r}")
+    return float(v)
+
+
+def fallback_rule(temperature, compression_ratio_threshold, logprob_threshold, top_k, vocab_size: int,
+                  default_top_k=None) -> Optional[Fallback]:
+    """Check the temperature-fallback arguments of ``transcribe``; the fallback to run, or None.
+
+    A schedule is a tuple or list of finite temperatures >= 0 (``None`` entries are 0.0) whose first entry is 0.0: the
+    first attempt is the window's ordinary decode.  A first entry above 0 raises ``NotImplementedError`` (as a scalar
+    temperature does); a negative, infinite or NaN entry ``ValueError``.  A fallback needs a schedule of two or more
+    entries and at least one threshold; with neither threshold, or with one entry, only the first entry runs (HF), and
+    ``compression_ratio_threshold`` without a schedule raises ``NotImplementedError``.  ``top_k``: the call's, else
+    ``default_top_k`` (the generation config's), else 50 (HF); 0 or at least ``vocab_size`` is the whole vocabulary, and
+    1 .. 64 is supported.  The call's ``top_k`` without a fallback to sample in raises ``NotImplementedError``, as an
+    option the engine does not honour.  Scalar temperatures are left to the caller's sampling refusal."""
+    no_sampling = NotImplementedError("top_k is only used by the sampled attempts of temperature fallback: pass a "
+                                      "temperature schedule and compression_ratio_threshold / logprob_threshold")
+    if not isinstance(temperature, (tuple, list)):
+        if compression_ratio_threshold is not None:
+            raise NotImplementedError("compression_ratio_threshold asks for temperature fallback: pass a temperature "
+                                      "schedule, e.g. temperature=(0.0, 0.2, 0.4, 0.6, 0.8, 1.0)")
+        if top_k is not None:
+            raise no_sampling
+        return None
+    if len(temperature) == 0:
+        raise ValueError("the temperature schedule is empty")
+    temps = tuple(0.0 if t is None else _finite("temperature", t) for t in temperature)
+    if any(t < 0 for t in temps):
+        raise ValueError(f"temperatures must be >= 0, got {temps}")
+    if temps[0] != 0.0:
+        raise NotImplementedError("sampling (temperature > 0 / do_sample) is not supported with medusa: the first entry "
+                                  "of a temperature schedule must be 0.0 (greedy search); sampling runs only on fallback")
+    crt = None if compression_ratio_threshold is None else _finite("compression_ratio_threshold", compression_ratio_threshold)
+    lpt = None if logprob_threshold is None else _finite("logprob_threshold", logprob_threshold)
+    if len(temps) == 1 or (crt is None and lpt is None):
+        if top_k is not None:
+            raise no_sampling
+        return None                 # HF: nothing to fall back to, the first entry is the decode
+    k = top_k if top_k is not None else (default_top_k if default_top_k is not None else 50)
+    if isinstance(k, bool) or not isinstance(k, (int, np.integer)) or k < 0:
+        raise ValueError(f"top_k must be a non-negative integer, got {k!r}")
+    k = 0 if int(k) >= vocab_size else int(k)
+    if k > MAX_TOP_K:
+        raise NotImplementedError(f"top_k must be at most {MAX_TOP_K}, 0 or at least the vocabulary size, got {k}")
+    return Fallback(temps, crt, lpt, k)
+
+
+def compression_ratio(ids: Sequence[int], vocab_size: int) -> float:
+    """HF ``_retrieve_compression_ratio``: the ids as little-endian integers of ``int(log2(vocab) / 8) + 1`` bytes, over
+    their zlib-compressed length."""
+    length = int(math.log2(vocab_size) / 8) + 1
+    token_bytes = b"".join(int(t).to_bytes(length, "little") for t in ids)
+    return len(token_bytes) / len(zlib.compress(token_bytes))
+
+
+def needs_fallback(ratio: float, avg_logprob: float, fb: Fallback) -> bool:
+    """HF ``_need_fallback`` without the no-speech rule: the compression ratio above its threshold, or the average
+    log-probability below its threshold (both strict)."""
+    return ((fb.compression_ratio_threshold is not None and ratio > fb.compression_ratio_threshold)
+            or (fb.logprob_threshold is not None and avg_logprob < fb.logprob_threshold))
+
+
 def resampled_length(n: int, orig_hz: int, new_hz: int) -> int:
     """``ceil(n * new / orig)`` with the rates divided by their gcd (torchaudio's output length)."""
     g = math.gcd(int(orig_hz), int(new_hz))
@@ -220,7 +302,8 @@ class WindowResult:
 
     def __init__(self, window: Window, ids: List[int], trace, no_speech_prob: Optional[float] = None,
                  avg_logprob: Optional[float] = None, skipped: Optional[bool] = None, token_timestamps=None,
-                 num_frames: Optional[int] = None):
+                 num_frames: Optional[int] = None, temperature: Optional[float] = None,
+                 compression_ratio: Optional[float] = None, attempts: Optional[List[Tuple[float, float, float]]] = None):
         self.start, self.end = window.start, window.end
         self.stride_left, self.stride_right = window.stride_left, window.stride_right
         self.ids = ids            # what generate() returns for the window (prompt and trailing EOS stripped)
@@ -232,6 +315,11 @@ class WindowResult:
         # transcribe(return_token_timestamps=True); both None without it
         self.token_timestamps = token_timestamps   # FloatTensor[1, len(ids)], seconds from the window's start
         self.num_frames = num_frames               # feature frames the alignment was cropped to
+        # temperature fallback (transcribe(temperature=(0.0, ...), ...)); all None without it: the kept attempt's
+        # temperature and compression ratio, and (temperature, compression_ratio, avg_logprob) of every attempt
+        self.temperature = temperature
+        self.compression_ratio = compression_ratio
+        self.attempts = attempts
 
     def merge_ids(self, eos_token_id: int) -> List[int]:
         """What the window contributes to ``merge_windows``: its text ids, or none for a skipped window (its

@@ -32,8 +32,9 @@ import torch
 
 from . import _lib
 from .config import MedusaConfig, MedusaGenerationConfig
-from .longform import (MAX_WINDOW_SAMPLES, SAMPLE_RATE, Window, WindowResult, merge_timed, merge_windows,
-                       no_speech_rule, plan_windows, resampled_length, skip_window, window_params)
+from .longform import (MAX_WINDOW_SAMPLES, SAMPLE_RATE, Fallback, Window, WindowResult, compression_ratio,
+                       fallback_rule, merge_timed, merge_windows, needs_fallback, no_speech_rule, plan_windows,
+                       resampled_length, skip_window, window_params)
 from . import processors as _processors
 from .weights import pack_blob
 
@@ -644,6 +645,7 @@ class WhisperMedusaModel:
                    language: Optional[str] = None, task: Optional[str] = None, temperature=None,
                    no_speech_threshold: Optional[float] = None, logprob_threshold: Optional[float] = None,
                    return_token_timestamps: Optional[bool] = None, time_precision: float = 0.02,
+                   compression_ratio_threshold: Optional[float] = None, top_k: Optional[int] = None,
                    **generate_kwargs) -> Union[torch.Tensor, MedusaGenerateOutput]:
         """Transcribe a mono recording of any length at any integer sampling rate; returns ``LongTensor[1, n]``.
 
@@ -663,7 +665,7 @@ class WhisperMedusaModel:
         the merge -- when the probability of ``<|nospeech|>`` at its start-of-transcript position is above
         ``no_speech_threshold`` and the average log-probability of its tokens is below ``logprob_threshold``.  Each
         window is still decoded in full (the rule needs its average log-probability).  ``no_speech_threshold`` alone
-        raises ``ValueError``; ``logprob_threshold`` alone (temperature fallback) ``NotImplementedError``.
+        raises ``ValueError``; ``logprob_threshold`` alone without a temperature schedule ``NotImplementedError``.
 
         ``return_token_timestamps=True``: a ``MedusaGenerateOutput`` whose ``sequences`` (``LongTensor[1, n]``) and
         ``token_timestamps`` (``FloatTensor[1, n, 2]``, the ``(start, end)`` of every id in seconds of the recording) are
@@ -673,24 +675,62 @@ class WhisperMedusaModel:
         the windows are merged by HF's timed rule, which matches overlapping ids only when their times are in order.
         The merged ids can therefore differ from those of the call without timestamps.  ``last_windows[i]`` holds each
         window's ``token_timestamps`` (relative to the window) and ``num_frames``.  The checks of ``generate``'s flag
-        (``alignment_heads``, filter width, a chain of ``medusa_choices``) run before anything is uploaded."""
+        (``alignment_heads``, filter width, a chain of ``medusa_choices``) run before anything is uploaded.
+
+        Temperature fallback (HF ``generate_with_fallback``): ``temperature`` a schedule such as ``(0.0, 0.2, 0.4, 0.6,
+        0.8, 1.0)`` whose first entry is 0.0, with ``compression_ratio_threshold`` and / or ``logprob_threshold``.  Each
+        window is first decoded as without the schedule; while its result has a compression ratio (HF's, over the
+        generated ids and the EOS) above ``compression_ratio_threshold`` or an average log-probability below
+        ``logprob_threshold``, it is decoded again from the same encoder output and prompt by sampling at the next
+        temperature, from the processed rows' top ``top_k`` entries (default: the generation config's, else 50; 0 = all;
+        at most 64).  The first attempt that passes is kept, else the last.  With ``no_speech_threshold`` the no-speech
+        rule skips a window instead and ends its attempts.  Sampling is reproducible under ``torch.manual_seed``: one
+        64-bit seed per recording is drawn from torch's default generator when a fallback is possible, and each
+        attempt's noise depends on (seed, window, attempt) only.  ``last_windows[i]`` records ``temperature``,
+        ``compression_ratio``, ``avg_logprob`` and ``attempts``.  Chains of ``medusa_choices`` only.  A one-entry schedule
+        takes the thresholds and never falls back (HF); ``top_k`` without a fallback raises ``NotImplementedError``."""
         self._require_engine()
         params = window_params(chunk_length_s, stride_length_s)
         _check_recording(audio, sampling_rate)
-        no_speech = ((float(no_speech_threshold), float(logprob_threshold))
-                     if no_speech_rule(no_speech_threshold, logprob_threshold) else None)
+        fallback, no_speech, temperature = self._fallback_request(temperature, compression_ratio_threshold,
+                                                                  logprob_threshold, no_speech_threshold, top_k)
         self._check_unsupported(temperature, None, generate_kwargs)
         self._logits_processors(generate_kwargs)
         if return_token_timestamps:
             self._timestamp_request(None, task, None, time_precision)
             generate_kwargs["time_precision"] = float(time_precision)
+        seed = self._recording_seed() if fallback is not None else None
         x16 = self._upload_16k(audio, sampling_rate)
         stream = torch.cuda.current_stream(self._device).cuda_stream
+        fb = {} if fallback is None else {"fallback": fallback}
         results = [self._transcribe_window(x16, w, stream, language=language, task=task, temperature=temperature,
-                                           no_speech=no_speech, **generate_kwargs)
-                   for w in plan_windows(x16.numel(), *params)]
+                                           no_speech=no_speech, **({"seed": (seed, i)} if fb else {}), **fb,
+                                           **generate_kwargs)
+                   for i, w in enumerate(plan_windows(x16.numel(), *params))]
         self.last_windows = results
         return self._merge_results(results, bool(return_token_timestamps))
+
+    def _fallback_request(self, temperature, compression_ratio_threshold, logprob_threshold, no_speech_threshold, top_k):
+        """Checks of ``transcribe``'s temperature-fallback and no-speech arguments before any GPU work: ``(fallback or
+        None, (no_speech_threshold, logprob_threshold) or None, the temperature left for the sampling refusal)``."""
+        fallback = fallback_rule(temperature, compression_ratio_threshold, logprob_threshold, top_k,
+                                 int(self.config.vocab_size), getattr(self.generation_config, "top_k", None))
+        if fallback is not None and any(int(c) != 1 for c in self.config.medusa_choices):
+            raise NotImplementedError("temperature fallback needs a chain of medusa_choices (all 1): sampled attempts "
+                                      "do not run on a branching tree")
+        # with a schedule, logprob_threshold without no_speech_threshold is a fallback threshold (a one-entry schedule
+        # has nothing to fall back to, as in HF); without one the rule refuses it as before
+        schedule = isinstance(temperature, (tuple, list))
+        lpt_rule = None if (schedule and no_speech_threshold is None) else logprob_threshold
+        no_speech = ((float(no_speech_threshold), float(logprob_threshold))
+                     if no_speech_rule(no_speech_threshold, lpt_rule) else None)
+        return fallback, no_speech, (None if isinstance(temperature, (tuple, list)) else temperature)
+
+    @staticmethod
+    def _recording_seed() -> Tuple[int, int]:
+        """One 64-bit seed of a recording's sampled attempts, as two 32-bit words, from torch's default generator."""
+        w = torch.randint(0, 2 ** 32, (2,), dtype=torch.int64)
+        return int(w[0]), int(w[1])
 
     def _merge_results(self, results: List[WindowResult], timed: bool) -> Union[torch.Tensor, MedusaGenerateOutput]:
         """The windows' merge: ``LongTensor[1, n]``, or with token timestamps the output of ``transcribe``."""
@@ -737,12 +777,16 @@ class WhisperMedusaModel:
 
     def _transcribe_window(self, x16: torch.Tensor, w: Window, producer_stream: int, language=None, task=None,
                            temperature=None, no_speech: Optional[Tuple[float, float]] = None,
-                           time_precision: Optional[float] = None, **kwargs) -> WindowResult:
+                           time_precision: Optional[float] = None, fallback: Optional[Fallback] = None,
+                           seed: Optional[Tuple[Tuple[int, int], int]] = None, **kwargs) -> WindowResult:
         """One window; ``no_speech`` = (no_speech_threshold, logprob_threshold) or None (the rule off);
-        ``time_precision`` = token timestamps with that precision, cropped to the window's frames, or None (off)."""
+        ``time_precision`` = token timestamps with that precision, cropped to the window's frames, or None (off);
+        ``fallback`` with ``seed`` = ((seed words of the recording), window index): temperature fallback, or None."""
         self._encode_window(x16, w, producer_stream)
         num_frames = None if time_precision is None else self.pcm_num_frames(w.end - w.start)
         ts = {} if time_precision is None else {"token_timestamps": (num_frames, float(time_precision))}
+        if fallback is not None:
+            return self._fallback_window(w, language, task, kwargs, no_speech, ts, num_frames, fallback, *seed)
         if no_speech is None:
             out = self._decode(language, task, kwargs, temperature, **ts)
             if not ts:
@@ -756,9 +800,48 @@ class WhisperMedusaModel:
                             skipped=skip_window(out.no_speech_prob, out.avg_logprob, *no_speech),
                             token_timestamps=out.token_timestamps, num_frames=num_frames)
 
+    def _fallback_window(self, w: Window, language, task, kwargs, no_speech, ts, num_frames, fb: Fallback,
+                         seed: Tuple[int, int], window_index: int) -> WindowResult:
+        """HF ``generate_with_fallback`` for one window whose encoder output is in place: attempts in schedule order
+        from the same prompt (the first one's: language detection runs once), until one does not need fallback or the
+        no-speech rule skips the window; the last attempt is kept when every one needs fallback."""
+        explicit = kwargs.pop("decoder_input_ids", None)
+        prompt = ([int(v) for v in torch.as_tensor(explicit).reshape(-1).tolist()] if explicit is not None
+                  else self._init_tokens(language, task))
+        attempts: List[Tuple[float, float, float]] = []
+        for a, t in enumerate(fb.temperatures):
+            kw = dict(kwargs, output_no_speech_prob=no_speech is not None, decoder_input_ids=prompt)
+            sampling = (t, fb.top_k, seed[0], seed[1], window_index, a) if t > 0 else None
+            if sampling is not None:
+                kw["medusa_temperature"] = 0.0       # exact-match acceptance against the sampled choices
+            out = self._decode(language, task, kw, None, return_dict_in_generate=True, sampling=sampling, **ts)
+            tr = self.last_trace
+            # HF's seek_sequence: the generated ids, up to and including the first EOS
+            ratio = compression_ratio(tr.sequences[len(prompt):len(prompt) + tr.n_new_tokens], int(self.config.vocab_size))
+            attempts.append((float(t), ratio, float(out.avg_logprob)))
+            skipped = no_speech is not None and skip_window(out.no_speech_prob, out.avg_logprob, *no_speech)
+            if skipped or not needs_fallback(ratio, out.avg_logprob, fb):
+                break
+        return WindowResult(w, out.sequences[0].tolist(), tr, no_speech_prob=out.no_speech_prob,
+                            avg_logprob=out.avg_logprob, skipped=skipped if no_speech is not None else None,
+                            token_timestamps=out.token_timestamps, num_frames=num_frames, temperature=float(t),
+                            compression_ratio=ratio, attempts=attempts)
+
+    def _push_sampling(self, sampling: Optional[Tuple[float, int, int, int, int, int]]) -> None:
+        """A sampled attempt's ``(temperature, top_k, seed_lo, seed_hi, window, attempt)``: sent on every sampled call
+        and switched off again on the engine that last had it, so other calls launch and draw nothing extra."""
+        if sampling is None and getattr(self, "_smp_engine", None) != self._handle.value:
+            return
+        lib = _lib.load()
+        t, k, lo, hi, win, att = sampling if sampling is not None else (0.0, 0, 0, 0, 0, 0)
+        _check(lib, self._handle, lib.wm_set_sampling(self._handle, float(t), int(k), lo, hi, win, att), "wm_set_sampling")
+        self._smp_engine = self._handle.value if sampling is not None else None
+
     def _decode(self, language, task, kwargs, temperature, generation_config=None, return_dict_in_generate=None,
-                token_timestamps: Optional[Tuple[Optional[int], float]] = None) -> Union[torch.Tensor, MedusaGenerateOutput]:
-        """``token_timestamps``: ``(num_frames or None, time_precision)`` from ``_timestamp_request``, or None."""
+                token_timestamps: Optional[Tuple[Optional[int], float]] = None,
+                sampling: Optional[Tuple[float, int, int, int, int, int]] = None) -> Union[torch.Tensor, MedusaGenerateOutput]:
+        """``token_timestamps``: ``(num_frames or None, time_precision)`` from ``_timestamp_request``, or None;
+        ``sampling``: a sampled attempt of temperature fallback (``_push_sampling``), or None."""
         g = generation_config if generation_config is not None else self.generation_config
         output_scores = bool(kwargs.pop("output_scores", False))
         output_logits = bool(kwargs.pop("output_logits", False))
@@ -812,6 +895,7 @@ class WhisperMedusaModel:
                    "wm_set_alignment_heads")
             self._ts_engine = self._handle.value if pairs else None
         self._push_logits_processors(procs)
+        self._push_sampling(sampling)
         tr = self._run_loop(prompt, gp)
         self.last_trace = tr
         self._last_medusa_temperature = float(gp.temperature)

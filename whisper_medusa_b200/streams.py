@@ -122,7 +122,7 @@ class StreamGroup:
         are merged in order.  The results equal ``model.transcribe`` of each recording, with the same
         ``no_speech_threshold`` / ``logprob_threshold`` rule and ``return_token_timestamps`` / ``time_precision`` (then
         one ``MedusaGenerateOutput`` per recording).  Per-window results: ``self.last_windows[i]`` for recording i."""
-        from .longform import no_speech_rule, plan_windows, window_params
+        from .longform import plan_windows, window_params
         from .model import _check_recording
 
         recs = [recordings] if isinstance(recordings, (np.ndarray, torch.Tensor)) else list(recordings)
@@ -132,23 +132,36 @@ class StreamGroup:
         params = window_params(chunk_length_s, stride_length_s)
         for r, sr in zip(recs, rates):
             _check_recording(r, sr)
-        nst, lpt = kwargs.pop("no_speech_threshold", None), kwargs.pop("logprob_threshold", None)
-        if no_speech_rule(nst, lpt):     # (same rule and arguments as model.transcribe)
-            kwargs["no_speech"] = (float(nst), float(lpt))
+        lead = self.models[0]
+        # (same rules and arguments as model.transcribe)
+        fallback, no_speech, temperature = lead._fallback_request(
+            kwargs.get("temperature"), kwargs.pop("compression_ratio_threshold", None),
+            kwargs.pop("logprob_threshold", None), kwargs.pop("no_speech_threshold", None), kwargs.pop("top_k", None))
+        if no_speech is not None:
+            kwargs["no_speech"] = no_speech
+        if fallback is not None:
+            kwargs["fallback"] = fallback
+        kwargs["temperature"] = temperature
         timed = bool(kwargs.pop("return_token_timestamps", None))
         time_precision = kwargs.pop("time_precision", 0.02)
-        lead = self.models[0]
-        lead._check_unsupported(kwargs.get("temperature"), None,
-                                {k: v for k, v in kwargs.items() if k not in ("language", "task", "temperature", "no_speech")})
+        lead._check_unsupported(temperature, None, {k: v for k, v in kwargs.items()
+                                                    if k not in ("language", "task", "temperature", "no_speech", "fallback")})
         lead._logits_processors(kwargs)
         if timed:
             lead._timestamp_request(None, kwargs.get("task"), None, time_precision)
             kwargs["time_precision"] = float(time_precision)
+        # one seed per recording, drawn in recording order: the same draws as model.transcribe of each in turn
+        seeds = [lead._recording_seed() for _ in recs] if fallback is not None else None
         x16 = [lead._upload_16k(r, sr) for r, sr in zip(recs, rates)]
         stream = torch.cuda.current_stream(self.device).cuda_stream     # every window's encode is ordered after it
-        items = [(i, w) for i, x in enumerate(x16) for w in plan_windows(x.numel(), *params)]
-        results = self._run(items, lambda m, it, kw: m._transcribe_window(x16[it[0]], it[1], stream, **kw), kwargs)
-        self.last_windows = [[res for (i, _), res in zip(items, results) if i == k] for k in range(len(recs))]
+        items = [(i, k, w) for i, x in enumerate(x16) for k, w in enumerate(plan_windows(x.numel(), *params))]
+
+        def window(m, it, kw):
+            seed = {"seed": (seeds[it[0]], it[1])} if seeds is not None else {}
+            return m._transcribe_window(x16[it[0]], it[2], stream, **seed, **kw)
+
+        results = self._run(items, window, kwargs)
+        self.last_windows = [[res for (i, _, _), res in zip(items, results) if i == k] for k in range(len(recs))]
         return [lead._merge_results(ws, timed) for ws in self.last_windows]
 
     def generate(self, input_features: torch.Tensor, **kwargs) -> List[torch.Tensor]:
