@@ -276,7 +276,8 @@ __device__ __forceinline__ float processed_logit(const float* row, int j, const 
   if ((mk & 1) || (begin_on && (mk & 2))) return -INFINITY;
   float v = ldcg_f(row + j);
   if (ADJ) v = v + ldcg_f(adj + j);
-  if (j == eos && pen != 0.f) v = v + fabsf(v) * pen;
+  // HF rounds the product and then the sum; a contracted FMA would round once and can differ in the last bit
+  if (j == eos && pen != 0.f) v = __fadd_rn(v, __fmul_rn(fabsf(v), pen));
   return v;
 }
 
