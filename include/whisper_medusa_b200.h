@@ -52,7 +52,13 @@ typedef struct wm_config {
   int32_t max_target_positions; /* 448 */
   int32_t medusa_num_heads;   /* K */
   int32_t medusa_block;       /* 0 = "base_head" (Medusa-Linear), 1 = "medusa_block" */
+  int32_t medusa_num_layers;  /* MedusaResBlocks per head, 1 .. WM_MAX_HEAD_LAYERS (reference model.py:235-246): heads_w /
+                               * heads_b hold layer l of every head at [l][head][d][d] / [l][head][d] */
 } wm_config;
+
+/* Most MedusaResBlocks per head wm_create accepts.  Each layer adds one head stage (and its grid barrier) to the
+ * candidate pass, and, for base_head, one to the verify pass. */
+#define WM_MAX_HEAD_LAYERS 4
 
 /* What _medusa_greedy_search reads from the generation config and kwargs
  * (reference model.py:404-835; medusa_utils.py:14-18). */
@@ -278,6 +284,10 @@ int wm_ring_schedule_check(int32_t d_model, int32_t n_layers, int32_t medusa_blo
  * yet copied never exceed the budget, and with a budget every copy was prefetched first. */
 int wm_ring_prefetch_check(int32_t d_model, int32_t n_layers, int32_t medusa_block, int32_t K, int32_t n_tree,
                            int32_t n_cta, int32_t l2_budget, int32_t* n_bad, int32_t* first4);
+/* wm_ring_schedule_check for heads of head_layers MedusaResBlocks each (1 .. WM_MAX_HEAD_LAYERS): one head stage per
+ * layer in the candidate pass, and for base_head in the verify pass. */
+int wm_ring_schedule_check_head_layers(int32_t d_model, int32_t n_layers, int32_t medusa_block, int32_t K, int32_t n_tree,
+                                       int32_t n_cta, int32_t head_layers, int32_t* n_bad, int32_t* first4);
 /* Debug: per-stage timeline of the last persistent iteration (after wm_set_option(h, "profile", 1)).
  * Rows of 24 int64: stage id, mode, layer; body ns and barrier-wait ns seen by the last CTA; then the
  * 16 raw probes of CTA 0 -- ns offsets from stage begin ([1] end of body, [2] end of barrier, [7] record

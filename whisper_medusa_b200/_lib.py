@@ -19,7 +19,9 @@ class EngineUnavailable(RuntimeError):
 class WmConfig(C.Structure):
     _fields_ = [(n, C.c_int32) for n in (
         "vocab_size", "d_model", "n_heads", "ffn_dim", "enc_layers", "dec_layers", "n_mels",
-        "max_source_positions", "max_target_positions", "medusa_num_heads", "medusa_block")]
+        "max_source_positions", "max_target_positions", "medusa_num_heads", "medusa_block", "medusa_num_layers")]
+
+WM_MAX_HEAD_LAYERS = 4   # include/whisper_medusa_b200.h
 
 
 class WmGenParams(C.Structure):
@@ -87,6 +89,8 @@ SYMBOLS = {
                                          _P(C.c_int32), _P(C.c_int32)]),
     "wm_ring_prefetch_check": (C.c_int, [C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                          _P(C.c_int32), _P(C.c_int32)]),
+    "wm_ring_schedule_check_head_layers": (C.c_int, [C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                                                     C.c_int32, _P(C.c_int32), _P(C.c_int32)]),
     "wm_set_option": (C.c_int, [C.c_void_p, C.c_char_p, C.c_int32]),
     "wm_get_stage_profile": (C.c_int, [C.c_void_p, _P(C.c_int64), C.c_int32, _P(C.c_int32)]),
 }

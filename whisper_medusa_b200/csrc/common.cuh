@@ -312,6 +312,8 @@ struct alignas(16) DecModel {   // (copied to shared memory in 16-byte pieces by
   int K;             // medusa heads
   int n_tree;        // rows of the verify pass: K+1 for the chain, tree nodes for branching medusa_choices
   int has_tree;      // 1 => branching choices: `tree` describes the candidate tree
+  int n_head_layers; // MedusaResBlocks per head (medusa_num_layers); fills the padding before `tree`, so the size and
+                     // every later offset of this struct are those of the single-layer layout
   const DecTree* tree;
   float* topk_part;  // [WM_MAX_T rows][32 segments][WM_TREE_MAX_TOPK]{value, index}: per-segment top-k of the tail scan
                      // (sampled attempts, which never have a tree: [WM_SMP_MAX_TOPK] entries per row and segment)
@@ -319,8 +321,8 @@ struct alignas(16) DecModel {   // (copied to shared memory in 16-byte pieces by
   const __half* embed;   // [V, d] (also proj_out)
   const float* pos;      // [max_target_positions, d]
   const float *lnf_g, *lnf_b;
-  const __half* heads_w; // [(K+1) or K][d, d]
-  const float* heads_b;
+  const __half* heads_w; // [n_head_layers][(K+1) or K][d, d], layer-major
+  const float* heads_b;  // [n_head_layers][(K+1) or K][d]
   const uint8_t* tok_mask;  // [V]: bit0 suppress, bit1 begin-suppress
   const float* pen_tab;     // [WM_MAX_POS + 32]: (factor^(L-start) - 1) as f32, 0 when inactive
   // activations (fp32)
@@ -330,7 +332,8 @@ struct alignas(16) DecModel {   // (copied to shared memory in 16-byte pieces by
   float* attn;     // [WM_MAX_T, d]
   float* ffn_h;    // [WM_MAX_T, ffn]
   float* hidden;   // [WM_MAX_T, d]  final-LN output (block type: input of the block)
-  float* head_h;   // [WM_MAX_T, d]
+  float* head_h;   // [2][WM_MAX_T, d]: head-layer outputs, ping-ponged between the halves (head_layer_out); the last
+                   // layer, and the block type's base row, are in the first half, which the vocabulary stage reads
   float* carry;    // [d] final-LN hidden state of the newest cached token (input of the heads)
   float* cross_part;  // [H][WM_CROSS_CHUNKS][WM_MAX_T][WM_HEAD_DIM + 2]
   int cross_chunks;   // key chunks per head of the cross-attention stage: clamp(n_sm / H, 1, 8)

@@ -79,7 +79,7 @@ __device__ __forceinline__ void stage_embed(const DecModel* m, int mode, int cta
 // skinny GEMM  y[t, n] = sum_k X[t, k] * W[n, k]   (t < 16 rows, W fp16 [N, K] row-major)
 // -----------------------------------------------------------------------------------------
 enum XSrc { XS_LN = 0, XS_PLAIN = 1 };
-enum Epi { EPI_QKV = 0, EPI_RESID, EPI_STORE, EPI_GELU, EPI_HEADS_A, EPI_HEAD_B, EPI_LOGITS };
+enum Epi { EPI_QKV = 0, EPI_RESID, EPI_STORE, EPI_GELU, EPI_HEADS_A, EPI_HEAD_B, EPI_LOGITS, EPI_HEADS_D };
 
 struct GemmDesc {
   const __half* W;
@@ -95,7 +95,7 @@ struct GemmDesc {
   int epi;
   float* out;          // EPI_STORE/GELU/LOGITS/HEAD*: destination [16, ldo]; EPI_RESID: residual stream
   int ldo;
-  int out_row0;        // EPI_HEADS_A: first destination row
+  int out_row0;        // EPI_HEADS_A / EPI_HEADS_D: destination row of head 0
   __half *kc, *vc;     // EPI_QKV: self K/V cache rows
   int base;            // EPI_QKV: cache row of token 0
   int d;               // model dim (EPI_QKV / EPI_HEADS_A)
@@ -155,6 +155,16 @@ __device__ __forceinline__ void gemm_epilogue(const GemmDesc& g, int token, int 
     case EPI_HEAD_B: {
       float xv = __half2float(xhi[(size_t)token * xstride + row]) + __half2float(xlo[(size_t)token * xstride + row]);
       g.out[(size_t)token * g.ldo + row] = xv + silu(v);
+      break;
+    }
+    case EPI_HEADS_D: {
+      // head layers after the first: head `row / d` on its own row of the previous layer (input row `head`); the
+      // other rows' products of its column block are discarded
+      int head = row / g.d, n = row - head * g.d;
+      if (token == head) {
+        float xv = __half2float(xhi[(size_t)token * xstride + n]) + __half2float(xlo[(size_t)token * xstride + n]);
+        g.out[(size_t)(g.out_row0 + head) * g.ldo + n] = xv + silu(v);
+      }
       break;
     }
   }
@@ -1523,6 +1533,13 @@ enum StageId {
 };
 enum PhaseId { PH_SWEEP_A = 0, PH_TAIL = 1, PH_VERIFY = 2 };
 
+// Output rows of head layer `layer`: the halves of head_h alternate from layer to layer, so that no layer writes rows
+// that a CTA may still be staging as its input, and the last layer is in the first half, where the vocabulary stage
+// reads (the block type's base row, stage_tail_seed / stage_final_ln, is there too)
+__host__ __device__ inline float* head_layer_out(const DecModel* m, int layer) {
+  return m->head_h + (size_t)((m->n_head_layers - 1 - layer) & 1) * WM_MAX_T * m->d;
+}
+
 // (host: called with the host copy of the model and an explicit geometry -- x_rows / base of the pass
 // are placeholders there, see dec_build_ring_tables)
 __host__ __device__ GemmDesc make_gemm_desc(const DecModel* m, int stage, int mode, int layer, const PassGeom* gopt) {
@@ -1573,20 +1590,32 @@ __host__ __device__ GemmDesc make_gemm_desc(const DecModel* m, int stage, int mo
       g.xsrc = XS_PLAIN; g.X = m->ffn_h;
       g.epi = EPI_RESID; g.out = m->x; g.ldo = d;
       break;
-    case ST_HEADS:
-      g.bias = m->heads_b; g.W = m->heads_w; g.K = d; g.xsrc = XS_PLAIN; g.out = m->head_h; g.ldo = d;
+    case ST_HEADS: {
+      // head layer `layer` (MedusaResBlock `layer` of every head, reference model.py:235-246): its weights are the
+      // layer-major stack's block `layer`
+      const int nh = m->has_block ? m->K : m->K + 1;
+      g.bias = m->heads_b + (size_t)layer * nh * d; g.W = m->heads_w + (size_t)layer * nh * d * d; g.K = d;
+      g.xsrc = XS_PLAIN; g.out = head_layer_out(m, layer); g.ldo = d;
       if (mode == MODE_A) {
-        // tail: every head on the hidden state of the newest token (generate_candidates reads
-        // logits[:, -1]); block type: on the medusa block's output for that token
-        g.X = m->has_block ? m->x : m->carry;
-        g.x_row0 = 0; g.x_rows = 1;
-        g.N = (m->has_block ? m->K : m->K + 1) * d;
-        g.epi = EPI_HEADS_A; g.out_row0 = m->has_block ? 1 : 0;
+        g.N = nh * d; g.out_row0 = m->has_block ? 1 : 0;
+        if (layer == 0) {
+          // tail: every head on the hidden state of the newest token (generate_candidates reads
+          // logits[:, -1]); block type: on the medusa block's output for that token
+          g.X = m->has_block ? m->x : m->carry;
+          g.x_row0 = 0; g.x_rows = 1;
+          g.epi = EPI_HEADS_A;
+        } else {
+          // later layers: each head on its own row of the previous layer's output
+          g.X = head_layer_out(m, layer - 1);
+          g.x_row0 = g.out_row0; g.x_rows = nh;
+          g.epi = EPI_HEADS_D;
+        }
       } else {
         // verify (base_head type only): head 0 on every tree position (disable_medusa, model.py:1281-1284)
-        g.X = m->hidden; g.N = d; g.epi = EPI_HEAD_B;
+        g.X = layer == 0 ? m->hidden : head_layer_out(m, layer - 1); g.N = d; g.epi = EPI_HEAD_B;
       }
       break;
+    }
     case ST_VOCAB:
     default:
       g.W = m->embed; g.N = m->V; g.K = d;
@@ -1659,17 +1688,19 @@ __host__ __device__ void seq_sweep(int n_layers, int has_block, int mode, F&& f)
   f(ST_FINAL_LN, mode, 0);
   if (has_block) { f(ST_COPY_HIDDEN, mode, 0); f(ST_QKV, mode, n_layers); }
 }
-// candidates from the carried hidden state: (block on it,) K+1 heads, vocab projection, top-1
+// candidates from the carried hidden state: (block on it,) K+1 heads (one stage per head layer), vocab projection, top-1
 template <class F>
-__host__ __device__ void seq_tail(int n_layers, int has_block, F&& f) {
+__host__ __device__ void seq_tail(int n_layers, int has_block, int n_head_layers, F&& f) {
   if (has_block) { f(ST_TAIL_SEED, MODE_TAIL, 0); seq_layer(n_layers, MODE_TAIL, f); }
-  f(ST_HEADS, MODE_A, 0); f(ST_VOCAB, MODE_A, 0); f(ST_SELECT1, MODE_A, 0); f(ST_SELECT_FIN, MODE_A, 0);
+  for (int l = 0; l < n_head_layers; ++l) f(ST_HEADS, MODE_A, l);
+  f(ST_VOCAB, MODE_A, 0); f(ST_SELECT1, MODE_A, 0); f(ST_SELECT_FIN, MODE_A, 0);
 }
 // verify: sweep B, base logits of the K+1 positions, acceptance statistics, accept
 template <class F>
-__host__ __device__ void seq_verify(int n_layers, int has_block, F&& f) {
+__host__ __device__ void seq_verify(int n_layers, int has_block, int n_head_layers, F&& f) {
   seq_sweep(n_layers, has_block, MODE_B, f);
-  if (!has_block) f(ST_HEADS, MODE_B, 0);
+  if (!has_block)
+    for (int l = 0; l < n_head_layers; ++l) f(ST_HEADS, MODE_B, l);
   f(ST_VOCAB, MODE_B, 0); f(ST_SELECT1, MODE_B, 0); f(ST_SELECT2, MODE_B, 0); f(ST_ACCEPT, MODE_B, 0);
   f(ST_KV_COMPACT, MODE_B, 0);   // (returns at once unless a candidate tree is configured)
 }
@@ -1746,8 +1777,8 @@ dec_iteration_kernel(const DecModel* __restrict__ m) {
   };
   if (need_a) seq_sweep(m->n_layers, m->has_block, MODE_A, run);
   if (!st->prefill) {   // (prefill: a 16-token chunk of a long prompt -- sweep A only)
-    seq_tail(m->n_layers, m->has_block, run);
-    seq_verify(m->n_layers, m->has_block, run);
+    seq_tail(m->n_layers, m->has_block, m->n_head_layers, run);
+    seq_verify(m->n_layers, m->has_block, m->n_head_layers, run);
   }
   if (blockIdx.x == 0 && threadIdx.x == 0) m->bar[2] = epoch;
 }
@@ -1759,15 +1790,15 @@ dec_iteration_kernel(const DecModel* __restrict__ m) {
 // -----------------------------------------------------------------------------------------
 // Flattened stage program {stage, mode, layer} x n, lists: [off0,off1) sweep A, [off1,off2) tail,
 // [off2,off3) verify -- what the ring kernel (consumer and producer side) walks.
-void dec_build_program(int n_layers, int has_block, std::vector<int>& flat, int off[4]) {
+void dec_build_program(int n_layers, int has_block, int n_head_layers, std::vector<int>& flat, int off[4]) {
   flat.clear();
   auto push = [&](int stage, int mode, int layer) { flat.push_back(stage); flat.push_back(mode); flat.push_back(layer); };
   off[0] = 0;
   seq_sweep(n_layers, has_block, MODE_A, push);
   off[1] = (int)flat.size() / 3;
-  seq_tail(n_layers, has_block, push);
+  seq_tail(n_layers, has_block, n_head_layers, push);
   off[2] = (int)flat.size() / 3;
-  seq_verify(n_layers, has_block, push);
+  seq_verify(n_layers, has_block, n_head_layers, push);
   off[3] = (int)flat.size() / 3;
 }
 
@@ -1835,7 +1866,7 @@ void dec_build_ring_tables(const DecModel& hm, const float2* ln_fold, int ncta, 
                            std::vector<ChunkDesc>& ctab, std::vector<int>& off) {
   std::vector<int> flat;
   int poff[4];
-  dec_build_program(hm.n_layers, hm.has_block, flat, poff);
+  dec_build_program(hm.n_layers, hm.has_block, hm.n_head_layers, flat, poff);
   const int n = poff[3];
   const PassGeom dyn{-1, 0};   // T = -1: "the rows of the pass" (resolved on the device)
   auto desc = [&](int ip) { return make_gemm_desc(&hm, flat[ip * 3], flat[ip * 3 + 1], flat[ip * 3 + 2], &dyn); };
@@ -1980,7 +2011,7 @@ int dec_check_ring_schedule(const DecModel& hm, int ncta, long long budget, int 
   dec_build_ring_tables(hm, fold, ncta, 1, stab, ctab, off);
   std::vector<int> flat;
   int poff[4];
-  dec_build_program(hm.n_layers, hm.has_block, flat, poff);
+  dec_build_program(hm.n_layers, hm.has_block, hm.n_head_layers, flat, poff);
   struct Copy {
     const void* src; uint32_t nrows, bytes;
     bool operator==(const Copy& o) const { return src == o.src && nrows == o.nrows && bytes == o.bytes; }
@@ -2219,8 +2250,8 @@ cudaError_t dec_enqueue_phase(const DecModel* dm, const DecHostInfo& hi, int pha
     if (n_launch) ++*n_launch;
   };
   if (phase == PH_SWEEP_A) seq_sweep(hi.n_layers, hi.has_block, MODE_A, launch);
-  else if (phase == PH_TAIL) seq_tail(hi.n_layers, hi.has_block, launch);
-  else seq_verify(hi.n_layers, hi.has_block, launch);
+  else if (phase == PH_TAIL) seq_tail(hi.n_layers, hi.has_block, hi.n_head_layers, launch);
+  else seq_verify(hi.n_layers, hi.has_block, hi.n_head_layers, launch);
   return cudaGetLastError();
 }
 

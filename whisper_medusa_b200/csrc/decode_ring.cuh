@@ -601,10 +601,12 @@ __device__ __forceinline__ void stage_gemm_ring(RingState& rs, unsigned char* sm
           if (row < D) out[(size_t)token * ldo + row] = v;
           else if (row < 2 * D) L.self_k[self_kv_index(base + token, row - D)] = __float2half_rn(v);
           else L.self_v[self_kv_index(base + token, row - 2 * D)] = __float2half_rn(v);
-        } else if (epi == EPI_HEADS_A) {
-          // head `row / d` on the newest token's hidden state: x + SiLU(W x + b)  (medusa ResBlock)
+        } else if (epi == EPI_HEADS_A || epi == EPI_HEADS_D) {
+          // head `row / d`: x + SiLU(W x + b)  (medusa ResBlock), on the newest token's hidden state (A: the one staged
+          // row) or, in later head layers, on its own row of the previous layer (D: row `head`, the others discarded)
           const int head = row / D, n = row - head * D;
-          out[(size_t)(sd->out_row0 + head) * ldo + n] = xbuf_value(xb, G::XS, 0, n) + silu(y);
+          if (epi == EPI_HEADS_A || token == head)
+            out[(size_t)(sd->out_row0 + head) * ldo + n] = xbuf_value(xb, G::XS, token, n) + silu(y);
         } else {   // EPI_HEAD_B
           out[(size_t)token * ldo + row] = xbuf_value(xb, G::XS, token, row) + silu(y);
         }

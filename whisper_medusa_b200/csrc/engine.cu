@@ -111,7 +111,7 @@ struct wm_handle {
   int st_from_generate = 0;   // 1 while `st` holds the last iteration of a completed wm_generate (wm_last_accept)
   // no-speech row (option "no_speech_row": index in the prompt of the SOT row, -1 = off); buffers allocated on first use
   int ns_prompt_row = -1;
-  float* ns_head = nullptr;     // [d] base_head type: the row after head 0
+  float* ns_head = nullptr;     // [2][d] base_head type: the row after each layer of head 0 (alternating halves)
   float* ns_logits = nullptr;   // [V] raw base-head logits of the row
   float* ns_part = nullptr;     // [WM_NS_NSEG][2] segment partials, then [1] log-sum-exp
   unsigned int* ns_count = nullptr;
@@ -205,9 +205,10 @@ static void build_layout(wm_handle* h) {
     add_tensor(h, p + "fc2_w", d * f, 0); add_tensor(h, p + "fc2_b", d, 1);
   }
   add_tensor(h, "dec.lnf_g", d, 1); add_tensor(h, "dec.lnf_b", d, 1);
+  // layer-major: [medusa_num_layers][nh][d][d] and [medusa_num_layers][nh][d]
   const size_t nh = c.medusa_block ? c.medusa_num_heads : c.medusa_num_heads + 1;
-  add_tensor(h, "heads_w", nh * d * d, 0);
-  add_tensor(h, "heads_b", nh * d, 1);
+  add_tensor(h, "heads_w", (size_t)c.medusa_num_layers * nh * d * d, 0);
+  add_tensor(h, "heads_b", (size_t)c.medusa_num_layers * nh * d, 1);
   h->wbytes = align_up(h->wbytes, 256);
 }
 
@@ -289,6 +290,7 @@ extern "C" int wm_create(const wm_config* cfg, int device, wm_handle** out) {
   if (c.ffn_dim % 128 != 0) return bad("ffn_dim must be a multiple of 128");
   if (c.n_mels != 80) return bad("n_mels must be 80");
   if (c.medusa_num_heads < 1 || c.medusa_num_heads + 1 > WM_MAX_T) return bad("medusa_num_heads must be in [1, 15]");
+  if (c.medusa_num_layers < 1 || c.medusa_num_layers > WM_MAX_HEAD_LAYERS) return bad("medusa_num_layers must be in [1, 4]");
   if (c.dec_layers + 1 > WM_MAX_DEC_LAYERS) return bad("too many decoder layers");
   if (c.max_target_positions + c.medusa_num_heads + 2 > WM_MAX_POS) return bad("max_target_positions too large");
   if (c.max_source_positions != 1500) return bad("max_source_positions must be 1500 (30 s window)");
@@ -341,7 +343,7 @@ extern "C" int wm_create(const wm_config* cfg, int device, wm_handle** out) {
   memset(&m, 0, sizeof m);
   m.d = (int)d; m.H = c.n_heads; m.ffn = (int)f; m.V = (int)V; m.S = h->S; m.S_pad = h->S_pad;
   m.n_layers = c.dec_layers; m.has_block = c.medusa_block ? 1 : 0; m.K = c.medusa_num_heads;
-  m.n_tree = c.medusa_num_heads + 1; m.has_tree = 0; m.tree = nullptr;
+  m.n_tree = c.medusa_num_heads + 1; m.has_tree = 0; m.tree = nullptr; m.n_head_layers = c.medusa_num_layers;
   CK(dalloc(&h->tree, 1));
   CK(dalloc(&m.topk_part, (size_t)WM_MAX_T * 32 * std::max(WM_TREE_MAX_TOPK, WM_SMP_MAX_TOPK) * 2));
   CK(dalloc(&m.x, (size_t)WM_MAX_T * d));
@@ -350,7 +352,7 @@ extern "C" int wm_create(const wm_config* cfg, int device, wm_handle** out) {
   CK(dalloc(&m.attn, (size_t)WM_MAX_T * d));
   CK(dalloc(&m.ffn_h, (size_t)WM_MAX_T * f));
   CK(dalloc(&m.hidden, (size_t)WM_MAX_T * d));
-  CK(dalloc(&m.head_h, (size_t)WM_MAX_T * d));
+  CK(dalloc(&m.head_h, (size_t)2 * WM_MAX_T * d));   // two halves: the head layers ping-pong (head_layer_out)
   CK(dalloc(&m.carry, d));
   CK(dalloc(&m.cross_part, (size_t)c.n_heads * WM_CROSS_CHUNKS * WM_MAX_T * (WM_HEAD_DIM + 2)));
   CK(dalloc(&m.cross_cnt, (size_t)c.n_heads));
@@ -375,6 +377,7 @@ extern "C" int wm_create(const wm_config* cfg, int device, wm_handle** out) {
 
   h->hi.n_sm = h->n_cta; h->hi.H = c.n_heads; h->hi.K = c.medusa_num_heads; h->hi.n_layers = c.dec_layers;
   h->hi.has_block = m.has_block;
+  h->hi.n_head_layers = m.n_head_layers;
   h->hi.n_tree = m.n_tree;
   h->hi.d = (int)d;
   h->hi.smem = dec_smem_bytes((int)d, (int)f);
@@ -384,7 +387,7 @@ extern "C" int wm_create(const wm_config* cfg, int device, wm_handle** out) {
   // product path by default: one persistent ring-kernel launch per speculative iteration.  Decoder widths the ring
   // kernel is not instantiated for (WM_RING_WIDTHS) fall back to the stage-kernel graphs.
   h->decode_mode = h->hi.smem_ring ? 2 : 0;
-  dec_build_program(c.dec_layers, m.has_block, h->prog, m.prog_off);
+  dec_build_program(c.dec_layers, m.has_block, m.n_head_layers, h->prog, m.prog_off);
   CK(enc_gemm_configure());
   h->tc_ok = (enc_gemm_tc_configure() == cudaSuccess);
   h->enc_gemm_impl = h->tc_ok ? 1 : 0;   // wgmma/TMA GEMM by default; option "enc_gemm" = 0 selects the mma.sync kernel
@@ -1045,6 +1048,8 @@ extern "C" int wm_generate(wm_handle* h, const int32_t* prompt, int32_t n_prompt
     na.hidden = h->hm.ns_hidden;
     na.head_w = h->hm.has_block ? nullptr : h->hm.heads_w;
     na.head_b = h->hm.heads_b;
+    na.head_layers = h->hm.n_head_layers;
+    na.head_stride = (size_t)(h->hm.K + 1) * h->hm.d;
     na.head_out = h->ns_head; na.embed = h->hm.embed; na.d = h->hm.d; na.V = h->hm.V;
     na.logits = h->ns_logits; na.part = h->ns_part; na.lse = h->ns_part + 2 * WM_NS_NSEG; na.count = h->ns_count;
     CK(dec_launch_no_speech(na, h->n_cta, s, &h->launches[2]));
@@ -1521,7 +1526,7 @@ extern "C" int wm_set_option(wm_handle* h, const char* key, int32_t value) {
     if (value >= 0 && !h->ns_logits) {
       CK(cudaStreamSynchronize(h->stream));   // (the device model description is rewritten below)
       CK(dalloc(&h->hm.ns_hidden, (size_t)h->hm.d));
-      CK(dalloc(&h->ns_head, (size_t)h->hm.d));
+      CK(dalloc(&h->ns_head, (size_t)2 * h->hm.d));
       CK(dalloc(&h->ns_logits, (size_t)h->cfg.vocab_size));
       CK(dalloc(&h->ns_part, (size_t)2 * WM_NS_NSEG + 1));
       CK(dalloc(&h->ns_count, 1));
@@ -1597,9 +1602,9 @@ extern "C" int wm_enc_gemm_tile(int32_t M, int32_t N, int32_t K, int32_t fp16_ou
   return WM_OK;
 }
 static int ring_check(int32_t d_model, int32_t n_layers, int32_t medusa_block, int32_t K, int32_t n_tree, int32_t n_cta,
-                      long long l2_budget, int32_t* n_bad, int32_t* first4) {
+                      long long l2_budget, int32_t* n_bad, int32_t* first4, int32_t head_layers = 1) {
   if (!n_bad || !first4 || d_model < 64 || d_model % 64 != 0 || n_layers < 1 || n_layers + 1 > WM_MAX_DEC_LAYERS || K < 1 ||
-      n_tree < 1 || n_tree > WM_MAX_T || n_cta < 4 || n_cta > 1024)
+      n_tree < 1 || n_tree > WM_MAX_T || n_cta < 4 || n_cta > 1024 || head_layers < 1 || head_layers > WM_MAX_HEAD_LAYERS)
     return WM_ERR_INVALID;
   // a model description whose buffers are distinct placeholder addresses (the replay compares addresses, never reads)
   uintptr_t next = uintptr_t(1) << 44;
@@ -1608,6 +1613,7 @@ static int ring_check(int32_t d_model, int32_t n_layers, int32_t medusa_block, i
   memset(&m, 0, sizeof m);
   m.d = d_model; m.H = d_model / 64; m.ffn = 4 * d_model; m.V = 51865; m.S = 1500; m.S_pad = 1536;
   m.n_layers = n_layers; m.has_block = medusa_block ? 1 : 0; m.K = K; m.n_tree = n_tree; m.has_tree = n_tree != K + 1;
+  m.n_head_layers = head_layers;
   m.cross_chunks = std::min(WM_CROSS_CHUNKS, std::max((m.S + WM_CH_MAX_KEYS - 1) / WM_CH_MAX_KEYS, n_cta / m.H));
   for (int i = 0; i < n_layers + m.has_block; ++i) {
     DecLayer& L = m.layers[i];
@@ -1630,5 +1636,10 @@ extern "C" int wm_ring_prefetch_check(int32_t d_model, int32_t n_layers, int32_t
   // a budget below one chunk would stall the cursor (the kernel's static_assert rules it out)
   if (l2_budget < 0 || (l2_budget > 0 && l2_budget < WM_RING_SLOT_MAX)) return WM_ERR_INVALID;
   return ring_check(d_model, n_layers, medusa_block, K, n_tree, n_cta, l2_budget, n_bad, first4);
+}
+extern "C" int wm_ring_schedule_check_head_layers(int32_t d_model, int32_t n_layers, int32_t medusa_block, int32_t K,
+                                                  int32_t n_tree, int32_t n_cta, int32_t head_layers, int32_t* n_bad,
+                                                  int32_t* first4) {
+  return ring_check(d_model, n_layers, medusa_block, K, n_tree, n_cta, -1, n_bad, first4, head_layers);
 }
 extern "C" void* wm_weights_device_ptr(wm_handle* h) { return (h && h->wready) ? (void*)h->wdev : nullptr; }

@@ -13,6 +13,7 @@ struct DecModel;
 struct DecHostInfo {
   int n_sm;
   int H, K, n_layers, has_block;
+  int n_head_layers;   // MedusaResBlocks per head
   int n_tree;      // rows of the verify pass (K + 1 for the chain)
   int d;
   size_t smem;
@@ -26,7 +27,7 @@ struct DecHostInfo {
 size_t dec_smem_bytes(int d, int ffn);
 cudaError_t dec_configure(int d, size_t smem, size_t smem_ring);
 size_t dec_ring_smem_bytes(int d);
-void dec_build_program(int n_layers, int has_block, std::vector<int>& flat, int off[4]);
+void dec_build_program(int n_layers, int has_block, int n_head_layers, std::vector<int>& flat, int off[4]);
 cudaError_t dec_relayout_cross_kv(const __half* kv, __half* ck, __half* cv, int S, int S_pad, int d, int H, cudaStream_t s,
                                   int64_t* n_launch);
 // {b'_n, c_n} of the LayerNorm-fed GEMMs of the ring kernel: float2 count for n_dec decoder layers, and the derivation
@@ -109,7 +110,9 @@ struct NoSpeechArgs {
   const float* hidden;     // [d] final-LayerNorm row captured by the loop (DecModel::ns_hidden)
   const __half* head_w;    // base_head type: head 0 [d, d] (the row goes through it first); null for medusa_block
   const float* head_b;     // [d]
-  float* head_out;         // [d] base_head type: hidden + SiLU(head_w . hidden + head_b)
+  int head_layers;         // base_head type: layers of head 0; layer l's weights at head_w + l * head_stride * d and
+  size_t head_stride;      // head_b + l * head_stride (head_stride = (K + 1) d rows per layer)
+  float* head_out;         // [2][d] base_head type: x + SiLU(W_l . x + b_l) after each layer l, in half l % 2
   const __half* embed;     // [V, d] proj_out (tied)
   int d, V;
   float* logits;           // [V] raw logits
@@ -117,8 +120,8 @@ struct NoSpeechArgs {
   float* lse;              // [1] log-sum-exp of the row
   unsigned int* count;     // arrival counter (zero between launches)
 };
-// grid: CTAs of each launch (<= decode_ctas); enqueues 2 kernels for the base_head type (head 0, then the vocabulary
-// product), 1 for medusa_block, and adds them to *n_launch
+// grid: CTAs of each launch (<= decode_ctas); enqueues head_layers + 1 kernels for the base_head type (each layer of
+// head 0, then the vocabulary product), 1 for medusa_block, and adds them to *n_launch
 cudaError_t dec_launch_no_speech(const NoSpeechArgs& a, int grid, cudaStream_t s, int64_t* n_launch);
 
 // ---- timestamps.cu ----

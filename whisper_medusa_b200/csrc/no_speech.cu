@@ -168,13 +168,24 @@ __global__ void __launch_bounds__(WM_NS_THREADS) no_speech_vocab_kernel(NoSpeech
 
 cudaError_t dec_launch_no_speech(const NoSpeechArgs& a, int grid, cudaStream_t s, int64_t* n_launch) {
   const size_t smem = (size_t)2 * a.d * sizeof(float);
+  NoSpeechArgs v = a;
   if (a.head_w) {
-    no_speech_head_kernel<<<std::max(1, std::min(grid, (a.d + NS_NW - 1) / NS_NW)), WM_NS_THREADS, smem, s>>>(a);
-    const cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return e;
-    ++*n_launch;
+    // one launch per layer of head 0, alternating between the halves of head_out: a layer's input row is staged by
+    // every CTA before any CTA of the next launch writes
+    for (int l = 0; l < a.head_layers; ++l) {
+      NoSpeechArgs al = a;
+      al.hidden = l == 0 ? a.hidden : a.head_out + (size_t)((l - 1) & 1) * a.d;
+      al.head_w = a.head_w + (size_t)l * a.head_stride * a.d;
+      al.head_b = a.head_b + (size_t)l * a.head_stride;
+      al.head_out = a.head_out + (size_t)(l & 1) * a.d;
+      no_speech_head_kernel<<<std::max(1, std::min(grid, (a.d + NS_NW - 1) / NS_NW)), WM_NS_THREADS, smem, s>>>(al);
+      const cudaError_t e = cudaGetLastError();
+      if (e != cudaSuccess) return e;
+      ++*n_launch;
+    }
+    v.head_out = a.head_out + (size_t)((a.head_layers - 1) & 1) * a.d;
   }
-  no_speech_vocab_kernel<<<std::max(1, std::min(grid, WM_NS_NSEG)), WM_NS_THREADS, smem, s>>>(a);
+  no_speech_vocab_kernel<<<std::max(1, std::min(grid, WM_NS_NSEG)), WM_NS_THREADS, smem, s>>>(v);
   ++*n_launch;
   return cudaGetLastError();
 }

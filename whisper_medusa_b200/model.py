@@ -237,7 +237,8 @@ class WhisperMedusaModel:
             vocab_size=c.vocab_size, d_model=c.d_model, n_heads=c.decoder_attention_heads, ffn_dim=c.decoder_ffn_dim,
             enc_layers=c.encoder_layers, dec_layers=c.decoder_layers, n_mels=c.num_mel_bins,
             max_source_positions=c.max_source_positions, max_target_positions=c.max_target_positions,
-            medusa_num_heads=c.medusa_num_heads, medusa_block=1 if c.is_block else 0)
+            medusa_num_heads=c.medusa_num_heads, medusa_block=1 if c.is_block else 0,
+            medusa_num_layers=c.medusa_num_layers)
 
     def to(self, device: Union[str, torch.device], broadcast_src: Optional[int] = None,
            weights_from: Optional["WhisperMedusaModel"] = None) -> "WhisperMedusaModel":

@@ -343,9 +343,9 @@ def synthetic_audio(seconds: float, stream_id: int = 0, seed: int = 1234) -> np.
     return x.astype(np.float32)
 
 
-def preset_config(name: str, heads: int = 10, heads_type: str = "base_head", **kw) -> MedusaConfig:
+def preset_config(name: str, heads: int = 10, heads_type: str = "base_head", head_layers: int = 1, **kw) -> MedusaConfig:
     """BASELINE.json configs: ``large-v2`` (cfg 2-5), ``tiny.en`` (cfg 1), ``micro`` (tests); ``base``, ``small`` and
-    ``medium`` (the full-depth tests)."""
+    ``medium`` (the full-depth tests).  ``head_layers``: MedusaResBlocks per head (``medusa_num_layers``)."""
     table = {
         "large-v2": "openai/whisper-large-v2",
         "tiny.en": "openai/whisper-tiny.en",
@@ -359,14 +359,15 @@ def preset_config(name: str, heads: int = 10, heads_type: str = "base_head", **k
 
     d_model = kw.get("d_model", WHISPER_PRESETS[wname]["d_model"])
     return MedusaConfig(
-        medusa_num_heads=heads, medusa_num_layers=1, medusa_hidden_size=d_model,
+        medusa_num_heads=heads, medusa_num_layers=head_layers, medusa_hidden_size=d_model,
         whisper_model_name=wname, medusa_choices=[1] * (heads + 1), medusa_heads_type=heads_type, **kw)
 
 
-def width_config(d_model: int, heads: int = 4, heads_type: str = "base_head", ffn_dim: int = 0) -> MedusaConfig:
+def width_config(d_model: int, heads: int = 4, heads_type: str = "base_head", ffn_dim: int = 0,
+                 head_layers: int = 1) -> MedusaConfig:
     """A small model at decoder width ``d_model``: micro's vocabulary and special tokens, 2 encoder and 2 decoder layers,
     d_model / 64 attention heads, FFN width ``ffn_dim`` (default 4 * d_model, as in every Whisper size)."""
     ffn = int(ffn_dim) or 4 * d_model
-    return preset_config("micro", heads=heads, heads_type=heads_type, d_model=d_model,
+    return preset_config("micro", heads=heads, heads_type=heads_type, head_layers=head_layers, d_model=d_model,
                          encoder_attention_heads=d_model // 64, decoder_attention_heads=d_model // 64,
                          encoder_ffn_dim=ffn, decoder_ffn_dim=ffn)

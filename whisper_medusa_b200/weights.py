@@ -12,7 +12,8 @@ engine tensor is derived from the HF/reference parameters (SURVEY.md 3.1 step 3)
   time-major activation (conv1's K = 240 is zero-padded to 256);
 * cross-attention k/v projections are fused into ``[2d, d]`` (the encoder-side GEMM writes the
   decode layout ``[pos][k | v]`` directly);
-* Medusa head linears are stacked ``[(K+1) d, d]`` (reference ``model.py:235-246``).
+* Medusa head linears are stacked layer-major, ``[L][(K+1) d, d]`` for ``L = medusa_num_layers`` ResBlocks per head
+  (reference ``model.py:235-246``); with one layer that is the ``[(K+1) d, d]`` stack of every head.
 Matrices stay fp16; vectors (biases, LayerNorm affine) and position tables are stored as fp32.
 """
 from __future__ import annotations
@@ -32,8 +33,8 @@ def engine_tensors(config: MedusaConfig, sd: Dict[str, torch.Tensor]):
     scale = float(config.head_dim) ** -0.5
     if config.head_dim != 64:
         raise NotImplementedError("the CUDA engine supports head_dim 64 only (every Whisper size)")
-    if config.medusa_num_layers != 1:
-        raise NotImplementedError("medusa_num_layers != 1 is not supported by the CUDA engine")
+    if not 1 <= config.medusa_num_layers <= _lib.WM_MAX_HEAD_LAYERS:
+        raise NotImplementedError(f"the CUDA engine supports medusa_num_layers 1 .. {_lib.WM_MAX_HEAD_LAYERS}")
     if config.medusa_hidden_size != d:
         raise ValueError("medusa_hidden_size must equal d_model (residual in MedusaResBlock, model.py:210)")
 
@@ -106,8 +107,9 @@ def engine_tensors(config: MedusaConfig, sd: Dict[str, torch.Tensor]):
     yield "dec.lnf_g", f32(f"{dec}.layer_norm.weight")
     yield "dec.lnf_b", f32(f"{dec}.layer_norm.bias")
     nh = config.medusa_num_heads + (0 if config.is_block else 1)
-    yield "heads_w", torch.cat([f16(f"medusa_heads.{i}.0.linear.weight") for i in range(nh)], 0)
-    yield "heads_b", torch.cat([f32(f"medusa_heads.{i}.0.linear.bias") for i in range(nh)], 0)
+    layers = range(config.medusa_num_layers)
+    yield "heads_w", torch.cat([f16(f"medusa_heads.{i}.{l}.linear.weight") for l in layers for i in range(nh)], 0)
+    yield "heads_b", torch.cat([f32(f"medusa_heads.{i}.{l}.linear.bias") for l in layers for i in range(nh)], 0)
 
 
 def pack_blob(handle, config: MedusaConfig, sd: Dict[str, torch.Tensor]) -> torch.Tensor:
